@@ -15,12 +15,6 @@ g++ -O2 -std=c++17 -fPIC -Wall -c $SRC/gsb_wire.cc -o build/gsb_wire.o
 g++ -O2 -std=c++17 -fPIC -Wall -c $SRC/gsb_fault.cc -o build/gsb_fault.o
 $NVCC -shared -gencode arch=compute_90a,code=sm_90a -cudart static -o $OUT build/hbm_probe_sm90a.o build/gsb_device.o build/gsb_wire.o build/gsb_fault.o -ldl -lpthread -lrt
 echo "built $OUT"
-if [ "${1:-}" = lab ]; then
-  # every tile shape / cache operator / L2 hint of the sweeps (tools/sweep_r02.py; GSB_LIB_PATH selects it)
-  $NVCC $FLAGS -DGSB_LAB=1 -c $SRC/hbm_probe_sm90a.cu -o build/hbm_probe_sm90a_lab.o
-  $NVCC -shared -gencode arch=compute_90a,code=sm_90a -cudart static -o $PKG/libgpushare_b200_lab.so build/hbm_probe_sm90a_lab.o build/gsb_device.o build/gsb_wire.o build/gsb_fault.o -ldl -lpthread -lrt
-  echo "built $PKG/libgpushare_b200_lab.so"
-fi
 # native daemon (C++ host side: HTTP/2 + HPACK gRPC front end, kube client, manager loop) + its h2 self-test
 g++ -O2 -std=c++17 -Wall -pthread -o $PKG/gsbd $SRC/daemon/gsbd.cc -L$PKG -lgpushare_b200 -lssl -lcrypto -ldl -Wl,-rpath,'$ORIGIN'
 g++ -O2 -std=c++17 -Wall -pthread -o build/h2_selftest $SRC/daemon/h2_selftest.cc

@@ -11,9 +11,7 @@ import ctypes as C
 import os
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
-# GSB_LIB_PATH: lab builds only (tools/sweep_r02.py loads libgpushare_b200_lab.so, the -DGSB_LAB=1 build that carries every
-# tile shape of the sweeps); the product, the tests and bench.py load the in-tree library
-LIB_PATH = os.environ.get("GSB_LIB_PATH") or os.path.join(_HERE, "libgpushare_b200.so")
+LIB_PATH = os.path.join(_HERE, "libgpushare_b200.so")
 
 GSB_UUID_BUFFER_SIZE = 80
 GSB_BUSID_BUFFER_SIZE = 32

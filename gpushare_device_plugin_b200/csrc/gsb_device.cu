@@ -160,7 +160,7 @@ struct Device {
   gsb_partial *partials = nullptr;
   unsigned int *ticket = nullptr;
   unsigned long long *tile_counter = nullptr;
-  uint32_t *seed_table = nullptr;  // device copy of gen[]
+  uint32_t *seed_table = nullptr;  // generation that last wrote each granule (written only by the kernels' last CTA)
   uint32_t launch_seq = 0;
   gsb_fault_log *fault_log = nullptr;                                // device memory: the kernels' fault log
   gsb_fault_log *fault_host = nullptr, *fault_host_dev = nullptr;    // mapped host copy a faulted launch leaves
@@ -170,7 +170,6 @@ struct Device {
   std::vector<Chunk> chunks;
   uint64_t arena_bytes = 0;
   std::map<uint64_t, gsb_launch_geom> geoms;  // (op, variant, grid request) -> resolved launch geometry
-  std::vector<uint32_t> gen;  // host mirror of seed_table: generation that last wrote each granule
   uint32_t next_gen = 1;
   bool faulted = false;  // prober: sticky
   std::vector<uint8_t> bits_scratch;  // Unhealthy bit string of this device's own list (faulted devices only)
@@ -409,7 +408,6 @@ int arena_destroy_locked(Device *d) {
   d->transient_arena = false;
   if (d->seed_table) cudaFree(d->seed_table);
   d->seed_table = nullptr;
-  d->gen.clear();
   return GSB_OK;
 }
 
@@ -480,7 +478,6 @@ int arena_create_locked(Device *d, uint64_t max_bytes, uint64_t keep_free, uint6
   }
   d->arena_bytes = mapped;
   const size_t n_gran = (size_t)((mapped + kGranuleBytes - 1) / kGranuleBytes);
-  d->gen.assign(n_gran, 0u);
   if (cudaMalloc(reinterpret_cast<void **>(&d->seed_table), n_gran * sizeof(uint32_t)) != cudaSuccess) {
     arena_destroy_locked(d);
     set_error("cudaMalloc(seed table) failed");
@@ -711,12 +708,6 @@ int probe_end_locked(Device *d, ProbeFlight *fl, gsb_probe_result *out) {
       out->kernel_ns = (uint64_t)((double)ms * 1e6);
     }
     if (ko.mismatch_words) store_fault_report(d, fl, out);
-    if (a.table_update) {  // host mirror of what the kernel's last CTA wrote
-      const uint64_t g0 = (cfg->window_offset + kGranuleBytes - 1) / kGranuleBytes;
-      const uint64_t g1 = (cfg->window_offset + fl->bytes) / kGranuleBytes;
-      const bool tail = cfg->window_offset + fl->bytes == d->arena_bytes && (d->arena_bytes % kGranuleBytes);
-      for (uint64_t g = g0; g < g1 + (tail ? 1 : 0) && g < d->gen.size(); g++) d->gen[g] = cfg->seed_write;
-    }
   }
   out->variant = fl->geom.variant;
   out->grid_ctas = fl->geom.grid;

@@ -57,7 +57,6 @@ struct gsb_kernel_args {
   unsigned long long arena_words; /* words in the whole arena (tail-granule rule of table_update) */
   uint32_t granule_shift;      /* log2(words per granule) */
   uint32_t launch_seq;
-  uint32_t l2_hint;            /* bit0: bulk loads carry an L2 evict_first policy, bit1: bulk stores do */
   uint32_t opaque_zero;        /* always 0; only the compiler does not know (DIRECT refill: a real load->store dependency) */
   gsb_partial *partials;       /* [grid] device memory */
   unsigned int *ticket;        /* device memory, self-resetting */

@@ -13,14 +13,12 @@
  *   CPASYNC  cp.async 16 B (LDGSTS) -> shared ring -> ld.shared.v4 -> st.global.v4
  *   BULK     cp.async.bulk (TMA 1-D, UBLKCP) + mbarrier -> shared ring -> ld.shared.v4 /
  *            st.shared.v4 -> cp.async.bulk shared->global
- * All are persistent grid-stride kernels over fixed-size tiles, grid = resident CTAs/SM x #SMs.
+ * All are persistent kernels over fixed-size tiles, grid = resident CTAs/SM x #SMs.
  *
- * What ships (default build): the two kernels GSB_VARIANT_AUTO ever launches — BULKD 32 KiB x 3 (FILL,
- * VERIFY_REFILL) and BULK 32 KiB x 3 (VERIFY) — plus ONE shape each of DIRECT, CPASYNC and BULKW, kept as
- * independent data paths for the parity tests (five implementations, one answer). The tile-shape / cache-operator /
- * L2-hint sweeps (72 kernel instantiations) are compiled only
- * with -DGSB_LAB=1 (build.sh lab -> libgpushare_b200_lab.so, used by tools/sweep_r02.py); in the default build the
- * GSB_*_CFG / GSB_DIRECT_FLAVOR / GSB_L2_HINT / GSB_DYN_FILL knobs are ignored.
+ * Kernels: the two GSB_VARIANT_AUTO launches — BULKD (FILL, VERIFY_REFILL) and BULK (VERIFY), one TMA ring with two
+ * tile schedules, 32 KiB x 3 stages — plus one shape each of DIRECT, CPASYNC and BULKW, kept as independent data
+ * paths for the parity tests (five implementations, one answer). Every shape is fixed at compile time; the H100
+ * tile-shape sweep behind the BULK / BULKD shape is in DESIGN.md §5.
  *
  * Reduction: per-thread registers -> warp shuffles -> one gsb_partial slot per CTA (plain stores,
  * no atomics on the data path) -> a self-resetting ticket elects the last CTA, which folds all
@@ -33,19 +31,13 @@
  */
 #include <cuda_runtime.h>
 #include <stdint.h>
-#include <stdlib.h>
 
 #include "gsb_internal.h"
 #include "gsb_pattern.h"
 
-#ifndef GSB_LAB
-#define GSB_LAB 0
-#endif
-
 namespace {
 
 constexpr int kThreads = 256;
-constexpr int kWarps = kThreads / 32;
 constexpr int kMaxWarps = 16;
 constexpr unsigned long long kNoBad = ~0ull;
 
@@ -69,23 +61,6 @@ __device__ __forceinline__ void st_stream(uint4 *p, const uint4 v) {
                "r"(v.w)
                : "memory");
 }
-// cache-operator flavours of the direct path (experiment knob GSB_DIRECT_FLAVOR, see DESIGN.md):
-// 0 = ld.cs/st.cs (streaming both ways), 1 = default ld/st, 2 = ld.L1::no_allocate + default st,
-// 3 = ld.cg/st.cg (L2 only)
-template <int F>
-__device__ __forceinline__ uint4 ld_flavor(const uint4 *p) {
-  uint4 v;
-  if (F == 0) {
-    return ld_stream(p);
-  } else if (F == 1) {
-    asm volatile("ld.global.v4.u32 {%0,%1,%2,%3}, [%4];" : "=r"(v.x), "=r"(v.y), "=r"(v.z), "=r"(v.w) : "l"(p) : "memory");
-  } else if (F == 2) {
-    asm volatile("ld.global.L1::no_allocate.v4.u32 {%0,%1,%2,%3}, [%4];" : "=r"(v.x), "=r"(v.y), "=r"(v.z), "=r"(v.w) : "l"(p) : "memory");
-  } else {
-    asm volatile("ld.global.cg.v4.u32 {%0,%1,%2,%3}, [%4];" : "=r"(v.x), "=r"(v.y), "=r"(v.z), "=r"(v.w) : "l"(p) : "memory");
-  }
-  return v;
-}
 // A refill stores to the address it has just loaded from, and the stored value (the next generation's pattern) does
 // not depend on the loaded one. Left alone, the four stores of a thread issue right behind its four loads, while
 // those loads are still in flight, and the memory system then orders every same-line load/store pair one at a time,
@@ -98,16 +73,6 @@ __device__ __forceinline__ uint4 ld_flavor(const uint4 *p) {
 __device__ __forceinline__ uint4 after_load(uint4 nw, uint32_t loaded, uint32_t opaque_zero) {
   nw.x ^= loaded & opaque_zero;
   return nw;
-}
-template <int F>
-__device__ __forceinline__ void st_flavor(uint4 *p, const uint4 v) {
-  if (F == 0) {
-    st_stream(p, v);
-  } else if (F == 3) {
-    asm volatile("st.global.cg.v4.u32 [%0], {%1,%2,%3,%4};" ::"l"(p), "r"(v.x), "r"(v.y), "r"(v.z), "r"(v.w) : "memory");
-  } else {
-    asm volatile("st.global.v4.u32 [%0], {%1,%2,%3,%4};" ::"l"(p), "r"(v.x), "r"(v.y), "r"(v.z), "r"(v.w) : "memory");
-  }
 }
 __device__ __forceinline__ uint32_t smem_u32(const void *p) {
   return static_cast<uint32_t>(__cvta_generic_to_shared(p));
@@ -127,6 +92,9 @@ __device__ __forceinline__ void mbar_init(uint32_t bar, uint32_t count) {
 __device__ __forceinline__ void mbar_expect_tx(uint32_t bar, uint32_t bytes) {
   asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(bar), "r"(bytes)
                : "memory");
+}
+__device__ __forceinline__ void mbar_arrive(uint32_t bar) {
+  asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(bar) : "memory");
 }
 __device__ __forceinline__ void mbar_wait(uint32_t bar, uint32_t parity) {
   asm volatile(
@@ -152,25 +120,6 @@ __device__ __forceinline__ void bulk_g2s(uint32_t dst_smem, const void *src, uin
 __device__ __forceinline__ void bulk_s2g(void *dst, uint32_t src_smem, uint32_t bytes) {
   asm volatile("cp.async.bulk.global.shared::cta.bulk_group [%0], [%1], %2;" ::"l"(dst), "r"(src_smem),
                "r"(bytes)
-               : "memory");
-}
-// same, carrying an L2 cache policy (createpolicy ... evict_first: streamed once, do not keep)
-__device__ __forceinline__ uint64_t l2_evict_first_policy() {
-  uint64_t p;
-  asm volatile("createpolicy.fractional.L2::evict_first.b64 %0, 1.0;" : "=l"(p));
-  return p;
-}
-__device__ __forceinline__ void bulk_g2s_hint(uint32_t dst_smem, const void *src, uint32_t bytes, uint32_t bar,
-                                              uint64_t policy) {
-  asm volatile(
-      "cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes.L2::cache_hint [%0], [%1], %2, [%3], %4;" ::"r"(
-          dst_smem),
-      "l"(src), "r"(bytes), "r"(bar), "l"(policy)
-      : "memory");
-}
-__device__ __forceinline__ void bulk_s2g_hint(void *dst, uint32_t src_smem, uint32_t bytes, uint64_t policy) {
-  asm volatile("cp.async.bulk.global.shared::cta.bulk_group.L2::cache_hint [%0], [%1], %2, %3;" ::"l"(dst),
-               "r"(src_smem), "r"(bytes), "l"(policy)
                : "memory");
 }
 __device__ __forceinline__ void bulk_commit() { asm volatile("cp.async.bulk.commit_group;" ::: "memory"); }
@@ -444,7 +393,7 @@ __device__ void finish(const gsb_kernel_args &a, const Acc &acc) {
 
 // ---------------------------------------------------------------- DIRECT
 
-template <int OP, int U, int F>
+template <int OP, int U>
 __global__ void __launch_bounds__(kThreads) probe_direct(const gsb_kernel_args a) {
   constexpr unsigned long long TILE = (unsigned long long)kThreads * U;
   const unsigned long long n_tiles = (a.n_words + TILE - 1) / TILE;
@@ -460,24 +409,24 @@ __global__ void __launch_bounds__(kThreads) probe_direct(const gsb_kernel_args a
     if ((t + 1) * TILE <= a.n_words) {
       if (OP != GSB_OP_FILL) {
 #pragma unroll
-        for (int u = 0; u < U; u++) v[u] = ld_flavor<F>(win + l0 + (unsigned long long)u * kThreads);
+        for (int u = 0; u < U; u++) v[u] = ld_stream(win + l0 + (unsigned long long)u * kThreads);
       }
 #pragma unroll
       for (int u = 0; u < U; u++) {
         const unsigned long long l = l0 + (unsigned long long)u * kThreads;
         uint4 nw = process_word<OP>(a, v[u], a.first_word + l, key_expect, key_write, acc);
         if (OP == GSB_OP_VERIFY_REFILL) nw = after_load(nw, v[u].x ^ v[u].y ^ v[u].z ^ v[u].w, a.opaque_zero);
-        if (OP != GSB_OP_VERIFY) st_flavor<F>(win + l, nw);
+        if (OP != GSB_OP_VERIFY) st_stream(win + l, nw);
       }
     } else {  // ragged last tile
 #pragma unroll
       for (int u = 0; u < U; u++) {
         const unsigned long long l = l0 + (unsigned long long)u * kThreads;
         if (l < a.n_words) {
-          if (OP != GSB_OP_FILL) v[u] = ld_flavor<F>(win + l);
+          if (OP != GSB_OP_FILL) v[u] = ld_stream(win + l);
           uint4 nw = process_word<OP>(a, v[u], a.first_word + l, key_expect, key_write, acc);
           if (OP == GSB_OP_VERIFY_REFILL) nw = after_load(nw, v[u].x ^ v[u].y ^ v[u].z ^ v[u].w, a.opaque_zero);
-          if (OP != GSB_OP_VERIFY) st_flavor<F>(win + l, nw);
+          if (OP != GSB_OP_VERIFY) st_stream(win + l, nw);
         }
       }
     }
@@ -538,37 +487,82 @@ __global__ void __launch_bounds__(kThreads) probe_cpasync(const gsb_kernel_args 
   finish(a, acc);
 }
 
-// ---------------------------------------------------------------- BULK (TMA 1-D ring)
+// ---------------------------------------------------------------- BULK / BULKD (TMA 1-D ring)
+//
+// One ring of S stages of TILE words. The leader (thread 0) starts the bulk load of slot k into stage k % S and
+// completes it on the stage's mbarrier; all threads process the tile in shared memory; the leader writes it back
+// with a bulk store. Which tile slot k holds is the schedule's business; the schedule is a template argument, so
+// nothing that differs between the two is decided at run time:
+//   has(k)      slot k is issued at all: the loop stops before waiting on a slot whose load was never issued
+//   next(k, s)  leader, once per slot in slot order: the tile slot k (stage s) holds, or the end of the walk
+//   tile(k, s)  every thread, after slot k's barrier: the same tile
+//   done(t)     t is the end of the walk
 
-template <int OP, int U, int S>
-__global__ void __launch_bounds__(kThreads) probe_bulk(const gsb_kernel_args a) {
+// BULK: slot k holds tile blockIdx + k * grid while k < my_n; every thread computes it.
+struct StaticSchedule {
+  unsigned long long my_n;
+  __device__ StaticSchedule(const gsb_kernel_args &, unsigned long long n_tiles, unsigned long long *)
+      : my_n(n_tiles > blockIdx.x ? (n_tiles - blockIdx.x + gridDim.x - 1) / gridDim.x : 0ull) {}
+  __device__ bool has(unsigned long long k) const { return k < my_n; }
+  __device__ unsigned long long next(unsigned long long k, int s) const { return tile(k, s); }
+  __device__ unsigned long long tile(unsigned long long k, int) const { return blockIdx.x + k * gridDim.x; }
+  __device__ static bool done(unsigned long long) { return false; }
+};
+
+// BULKD: the leader claims the next tile from an atomic counter when it issues a slot, so CTAs that run ahead simply
+// take more tiles and the kernel ends with every CTA busy (no straggler tail). Claims are made in time order, so
+// concurrently processed tiles stay neighbours in memory. The claimed index travels to the consumers through
+// tile_of[s] under the stage's mbarrier (arrive = release, wait = acquire); every slot is issued, and the first one
+// past the last tile holds kDone.
+struct ClaimedSchedule {
+  static constexpr unsigned long long kDone = ~0ull;
+  unsigned long long n_tiles, in_hand = 0;
+  unsigned long long *counter, *tile_of;
+  __device__ ClaimedSchedule(const gsb_kernel_args &a, unsigned long long n, unsigned long long *slots)
+      : n_tiles(n), counter(a.tile_counter), tile_of(slots) {
+    // the leader always holds one claim in hand: the atomic for the NEXT tile is issued when the current one is
+    // consumed, so its ~L2 round trip overlaps the tile being processed instead of delaying the next load
+    if (threadIdx.x == 0) in_hand = atomicAdd(counter, 1ull);
+  }
+  __device__ bool has(unsigned long long) const { return true; }
+  __device__ unsigned long long next(unsigned long long, int s) {
+    const unsigned long long t = in_hand;
+    in_hand = atomicAdd(counter, 1ull);
+    return tile_of[s] = t < n_tiles ? t : kDone;
+  }
+  __device__ unsigned long long tile(unsigned long long, int s) const { return tile_of[s]; }
+  __device__ static bool done(unsigned long long t) { return t == kDone; }
+};
+
+template <int OP, int U, int S, typename Schedule>
+__device__ __forceinline__ void bulk_ring(const gsb_kernel_args &a) {
   constexpr unsigned long long TILE = (unsigned long long)kThreads * U;
   extern __shared__ __align__(128) unsigned char smem_raw[];
   uint4 *ring = reinterpret_cast<uint4 *>(smem_raw);  // [S][TILE]
   __shared__ __align__(8) unsigned long long full_bar[S];
+  __shared__ unsigned long long tile_of[S];  // ClaimedSchedule only
   const unsigned long long n_tiles = (a.n_words + TILE - 1) / TILE;
-  const unsigned long long my_n =
-      n_tiles > blockIdx.x ? (n_tiles - blockIdx.x + gridDim.x - 1) / gridDim.x : 0ull;
+  Schedule sched(a, n_tiles, tile_of);
   const uint32_t key_write = gsb_seed_key(a.seed_write);
   uint4 *__restrict__ win = a.base + a.first_word;
   const bool leader = threadIdx.x == 0;
-  const uint64_t policy = a.l2_hint ? l2_evict_first_policy() : 0ull;
   Acc acc;
 
-  auto tile_words = [&](unsigned long long k) -> uint32_t {
-    const unsigned long long t = blockIdx.x + k * gridDim.x;
+  auto words_of = [&](unsigned long long t) -> uint32_t {
     const unsigned long long left = a.n_words - t * TILE;
     return (uint32_t)(left < TILE ? left : TILE);
   };
-  auto load = [&](unsigned long long k) {  // leader only
-    const unsigned long long t = blockIdx.x + k * gridDim.x;
+  auto load = [&](unsigned long long k) {  // leader only: issue slot k
+    if (!sched.has(k)) return;
     const int s = (int)(k % S);
-    const uint32_t bytes = tile_words(k) * 16u;
+    const unsigned long long t = sched.next(k, s);
+    if (Schedule::done(t)) {
+      mbar_arrive(smem_u32(&full_bar[s]));  // no tile: the consumers still pass the barrier, and read kDone
+      return;
+    }
+    const uint32_t bytes = words_of(t) * 16u;
     mbar_expect_tx(smem_u32(&full_bar[s]), bytes);
-    if (a.l2_hint & 1u)
-      bulk_g2s_hint(smem_u32(ring + s * TILE), win + t * TILE, bytes, smem_u32(&full_bar[s]), policy);
-    else
-      bulk_g2s(smem_u32(ring + s * TILE), win + t * TILE, bytes, smem_u32(&full_bar[s]));
+    bulk_g2s(smem_u32(ring + s * TILE), win + t * TILE, bytes, smem_u32(&full_bar[s]));
   };
 
   fault_smem_init();
@@ -582,23 +576,24 @@ __global__ void __launch_bounds__(kThreads) probe_bulk(const gsb_kernel_args a) 
   // prologue: VERIFY can keep all S stages in flight (a consumed stage is refilled at once);
   // VERIFY_REFILL keeps S-1 (a stage is refilled one iteration after its store was issued)
   constexpr int kPrologue = (OP == GSB_OP_VERIFY) ? S : S - 1;
-  if (OP != GSB_OP_FILL && leader) {
-    for (int k = 0; k < kPrologue; k++)
-      if ((unsigned long long)k < my_n) load(k);
-  }
+  if (OP != GSB_OP_FILL && leader)
+    for (int k = 0; k < kPrologue; k++) load(k);
 
-  for (unsigned long long k = 0; k < my_n; k++) {
-    const unsigned long long t = blockIdx.x + k * gridDim.x;
+  for (unsigned long long k = 0; sched.has(k); k++) {
     const int s = (int)(k % S);
-    const uint32_t nw_tile = tile_words(k);
-    uint4 *stage = ring + s * TILE;
     if (OP == GSB_OP_FILL) {
-      // the bulk store that last read this stage (tile k-S) must have drained it
-      if (leader) bulk_wait_read<S - 1>();
+      if (leader) {
+        bulk_wait_read<S - 1>();  // the bulk store that last read this stage (slot k-S) has drained it
+        sched.next(k, s);
+      }
       __syncthreads();
     } else {
       mbar_wait(smem_u32(&full_bar[s]), (uint32_t)((k / S) & 1ull));
     }
+    const unsigned long long t = sched.tile(k, s);
+    if (Schedule::done(t)) break;  // uniform: every thread reads the same slot after the same barrier
+    const uint32_t nw_tile = words_of(t);
+    uint4 *stage = ring + s * TILE;
     const uint32_t key_expect = (OP != GSB_OP_FILL) ? expect_key_of(a, a.first_word + t * TILE) : 0u;
 #pragma unroll
     for (int u = 0; u < U; u++) {
@@ -614,14 +609,11 @@ __global__ void __launch_bounds__(kThreads) probe_bulk(const gsb_kernel_args a) 
     __syncthreads();  // every thread is done with this stage (reads, and writes + proxy fence)
     if (leader) {
       if (OP == GSB_OP_VERIFY) {
-        if (k + S < my_n) load(k + S);  // same stage, just released by the barrier
+        load(k + S);  // same stage, just released by the barrier
       } else {
-        if (a.l2_hint & 2u)
-          bulk_s2g_hint(win + t * TILE, smem_u32(stage), nw_tile * 16u, policy);
-        else
-          bulk_s2g(win + t * TILE, smem_u32(stage), nw_tile * 16u);
+        bulk_s2g(win + t * TILE, smem_u32(stage), nw_tile * 16u);
         bulk_commit();
-        if (OP == GSB_OP_VERIFY_REFILL && k + S - 1 < my_n) {
+        if (OP == GSB_OP_VERIFY_REFILL && sched.has(k + S - 1)) {
           // refill stage (k-1)%S: its store (tile k-1) must have finished READING shared memory;
           // one group (tile k's store, just committed) may stay in flight
           if (k >= 1) bulk_wait_read<1>();
@@ -634,106 +626,14 @@ __global__ void __launch_bounds__(kThreads) probe_bulk(const gsb_kernel_args a) 
   finish(a, acc);
 }
 
-// ---------------------------------------------------------------- BULKD (TMA ring, dynamic tile scheduler)
-//
-// BULK with the static stride (tile = blockIdx + k*grid) replaced by an atomic tile counter: the leader
-// claims the next tile when it issues that tile's load, so CTAs that run ahead simply take more tiles and
-// the kernel ends with every CTA busy (no straggler tail). Claims are made in time order, so concurrently
-// processed tiles stay neighbours in memory. The claimed index travels to the consumers through shared
-// memory under the stage's mbarrier (arrive = release, wait = acquire).
+template <int OP, int U, int S>
+__global__ void __launch_bounds__(kThreads) probe_bulk(const gsb_kernel_args a) {
+  bulk_ring<OP, U, S, StaticSchedule>(a);
+}
+
 template <int OP, int U, int S>
 __global__ void __launch_bounds__(kThreads) probe_bulk_dyn(const gsb_kernel_args a) {
-  constexpr unsigned long long TILE = (unsigned long long)kThreads * U;
-  constexpr unsigned long long kDone = ~0ull;
-  extern __shared__ __align__(128) unsigned char smem_raw[];
-  uint4 *ring = reinterpret_cast<uint4 *>(smem_raw);  // [S][TILE]
-  __shared__ __align__(8) unsigned long long full_bar[S];
-  __shared__ unsigned long long tile_of[S];
-  const unsigned long long n_tiles = (a.n_words + TILE - 1) / TILE;
-  const uint32_t key_write = gsb_seed_key(a.seed_write);
-  uint4 *__restrict__ win = a.base + a.first_word;
-  const bool leader = threadIdx.x == 0;
-  Acc acc;
-  // the leader always holds one claim in hand: the atomic for the NEXT tile is issued when the current one
-  // is consumed, so its ~L2 round trip overlaps the tile being processed instead of delaying the next load
-  unsigned long long in_hand = 0;
-  if (leader) in_hand = atomicAdd(a.tile_counter, 1ull);
-  auto claim = [&]() -> unsigned long long {
-    const unsigned long long t = in_hand;
-    in_hand = atomicAdd(a.tile_counter, 1ull);
-    return t < n_tiles ? t : kDone;
-  };
-  auto words_of = [&](unsigned long long t) -> uint32_t {
-    const unsigned long long left = a.n_words - t * TILE;
-    return (uint32_t)(left < TILE ? left : TILE);
-  };
-  auto load_next = [&](unsigned long long k) {  // leader only: claim a tile for slot k and start its load
-    const int s = (int)(k % S);
-    const unsigned long long t = claim();
-    tile_of[s] = t;
-    if (t != kDone) {
-      const uint32_t bytes = words_of(t) * 16u;
-      mbar_expect_tx(smem_u32(&full_bar[s]), bytes);
-      bulk_g2s(smem_u32(ring + s * TILE), win + t * TILE, bytes, smem_u32(&full_bar[s]));
-    } else {
-      asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(smem_u32(&full_bar[s])) : "memory");
-    }
-  };
-
-  fault_smem_init();
-  if (leader) {
-#pragma unroll
-    for (int s = 0; s < S; s++) mbar_init(smem_u32(&full_bar[s]), 1u);
-    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-  }
-  __syncthreads();
-  constexpr int kPrologue = (OP == GSB_OP_VERIFY) ? S : S - 1;
-  if (OP != GSB_OP_FILL && leader)
-    for (int k = 0; k < kPrologue; k++) load_next(k);
-
-  for (unsigned long long k = 0;; k++) {
-    const int s = (int)(k % S);
-    if (OP == GSB_OP_FILL) {
-      if (leader) {
-        bulk_wait_read<S - 1>();  // the store that last read this stage (slot k-S) has drained it
-        tile_of[s] = claim();
-      }
-      __syncthreads();
-    } else {
-      mbar_wait(smem_u32(&full_bar[s]), (uint32_t)((k / S) & 1ull));
-    }
-    const unsigned long long t = tile_of[s];
-    if (t == kDone) break;  // uniform: every thread reads the same slot after the same barrier
-    const uint32_t nw_tile = words_of(t);
-    uint4 *stage = ring + s * TILE;
-    const uint32_t key_expect = (OP != GSB_OP_FILL) ? expect_key_of(a, a.first_word + t * TILE) : 0u;
-#pragma unroll
-    for (int u = 0; u < U; u++) {
-      const uint32_t i = u * kThreads + threadIdx.x;
-      if (i < nw_tile) {
-        uint4 v = make_uint4(0, 0, 0, 0);
-        if (OP != GSB_OP_FILL) v = stage[i];
-        const uint4 nw = process_word<OP>(a, v, a.first_word + t * TILE + i, key_expect, key_write, acc);
-        if (OP != GSB_OP_VERIFY) stage[i] = nw;
-      }
-    }
-    if (OP != GSB_OP_VERIFY) fence_proxy_async_smem();
-    __syncthreads();
-    if (leader) {
-      if (OP == GSB_OP_VERIFY) {
-        load_next(k + S);
-      } else {
-        bulk_s2g(win + t * TILE, smem_u32(stage), nw_tile * 16u);
-        bulk_commit();
-        if (OP == GSB_OP_VERIFY_REFILL) {
-          if (k >= 1) bulk_wait_read<1>();  // stage (k-1)%S: its store has finished reading shared memory
-          load_next(k + S - 1);
-        }
-      }
-    }
-  }
-  if (leader && OP != GSB_OP_VERIFY) bulk_wait_all<0>();
-  finish(a, acc);
+  bulk_ring<OP, U, S, ClaimedSchedule>(a);
 }
 
 // ---------------------------------------------------------------- BULKW (per-warp TMA rings)
@@ -760,7 +660,6 @@ __global__ void __launch_bounds__(WARPS * 32) probe_bulk_warp(const gsb_kernel_a
   const uint32_t key_write = gsb_seed_key(a.seed_write);
   uint4 *__restrict__ win = a.base + a.first_word;
   const bool leader = lane == 0;
-  const uint64_t policy = a.l2_hint ? l2_evict_first_policy() : 0ull;
   Acc acc;
 
   auto tile_words = [&](unsigned long long k) -> uint32_t {
@@ -771,10 +670,7 @@ __global__ void __launch_bounds__(WARPS * 32) probe_bulk_warp(const gsb_kernel_a
     const int s = (int)(k % S);
     const uint32_t bytes = tile_words(k) * 16u;
     mbar_expect_tx(smem_u32(&full_bar[warp][s]), bytes);
-    if (a.l2_hint & 1u)
-      bulk_g2s_hint(smem_u32(ring + s * TILE), win + tile_of(k) * TILE, bytes, smem_u32(&full_bar[warp][s]), policy);
-    else
-      bulk_g2s(smem_u32(ring + s * TILE), win + tile_of(k) * TILE, bytes, smem_u32(&full_bar[warp][s]));
+    bulk_g2s(smem_u32(ring + s * TILE), win + tile_of(k) * TILE, bytes, smem_u32(&full_bar[warp][s]));
   };
 
   fault_smem_init();
@@ -832,10 +728,7 @@ __global__ void __launch_bounds__(WARPS * 32) probe_bulk_warp(const gsb_kernel_a
       if (OP == GSB_OP_VERIFY) {
         if (k + S < my_n) load(k + S);
       } else {
-        if (a.l2_hint & 2u)
-          bulk_s2g_hint(win + t * TILE, smem_u32(stage), nw_tile * 16u, policy);
-        else
-          bulk_s2g(win + t * TILE, smem_u32(stage), nw_tile * 16u);
+        bulk_s2g(win + t * TILE, smem_u32(stage), nw_tile * 16u);
         bulk_commit();
         if (OP == GSB_OP_VERIFY_REFILL && k + S - 1 < my_n) {
           if (k >= 1) bulk_wait_read<1>();
@@ -851,9 +744,14 @@ __global__ void __launch_bounds__(WARPS * 32) probe_bulk_warp(const gsb_kernel_a
 // ---------------------------------------------------------------- geometry + dispatch
 
 constexpr int kDirectU = 4;
-constexpr int kCpU = 4, kCpS = 4;      // 16 KiB tiles x 4 stages = 64 KiB / CTA
-constexpr int kBulkU = 4, kBulkS = 4;  // 16 KiB tiles x 4 stages = 64 KiB / CTA
+constexpr int kCpU = 4, kCpS = 4;  // 16 KiB tiles x 4 stages = 64 KiB / CTA
+// 32 KiB tiles x 3 stages = 96 KiB / CTA: 2 CTAs per H100 SM (228 KiB); no other shape of the H100 sweep was more
+// than ~1 % faster for any op (DESIGN.md §5)
+constexpr int kBulkU = 8, kBulkS = 3;
+constexpr int kBulkwWpl = 8, kBulkwS = 3, kBulkwWarps = 8;  // 4 KiB warp-tiles x 3 stages x 8 warps = 96 KiB / CTA
 constexpr uint32_t kCpSmem = kCpU * kThreads * 16 * kCpS;
+constexpr uint32_t kBulkSmem = kBulkU * kThreads * 16 * kBulkS;
+constexpr uint32_t kBulkwSmem = kBulkwWpl * 512 * kBulkwS * kBulkwWarps;
 constexpr int kMaxCtasPerSm = 8;
 
 template <typename K>
@@ -869,174 +767,40 @@ int resident_ctas(K kernel, uint32_t smem, int threads) {
 
 typedef void (*probe_fn)(const gsb_kernel_args);
 
-// knob GSB_DYN_FILL=0: FILL under GSB_VARIANT_BULKD falls back to the static kernel (32 KiB x 6)
-bool dyn_fill() {
-#if GSB_LAB
-  static const bool f = [] {
-    const char *e = getenv("GSB_DYN_FILL");
-    return !e || atoi(e) != 0;
-  }();
-  return f;
-#else
-  return true;
-#endif
+probe_fn by_op(uint32_t op, probe_fn fill, probe_fn verify, probe_fn verify_refill) {
+  if (op == GSB_OP_FILL) return fill;
+  if (op == GSB_OP_VERIFY) return verify;
+  if (op == GSB_OP_VERIFY_REFILL) return verify_refill;
+  return nullptr;
 }
 
-// experiment knob GSB_BULKW_CFG: warp-tile size x ring depth x warps per CTA of the per-warp TMA path
-int bulkw_cfg() {
-#if !GSB_LAB
-  return 0;
-#endif
-  static const int f = [] {
-    const char *e = getenv("GSB_BULKW_CFG");
-    const int v = e ? atoi(e) : 0;
-    return v < 0 || v > 7 ? 0 : v;
-  }();
-  return f;
-}
-
-// experiment knob GSB_BULK_CFG: tile size x ring depth of the TMA path (unset = per-op default)
-int bulk_cfg() {
-#if !GSB_LAB
-  return -1;
-#endif
-  static const int f = [] {
-    const char *e = getenv("GSB_BULK_CFG");
-    const int v = e ? atoi(e) : -1;
-    return v < 0 || v > 8 ? -1 : v;
-  }();
-  return f;
-}
-
-// experiment knob GSB_L2_HINT: bit0 loads / bit1 stores of the TMA paths carry L2::evict_first
-uint32_t l2_hint_knob() {
-#if !GSB_LAB
-  return 0u;
-#endif
-  static const uint32_t f = [] {
-    const char *e = getenv("GSB_L2_HINT");
-    return e ? (uint32_t)atoi(e) & 3u : 0u;
-  }();
-  return f;
-}
-
-int direct_flavor() {
-#if !GSB_LAB
-  return 0;
-#endif
-  static const int f = [] {
-    const char *e = getenv("GSB_DIRECT_FLAVOR");
-    const int v = e ? atoi(e) : 0;
-    return v < 0 || v > 3 ? 0 : v;
-  }();
-  return f;
-}
-
+// the kernel of (op, variant), its dynamic shared memory and block size; nullptr if there is none
 probe_fn pick(uint32_t op, uint32_t variant, uint32_t *smem, uint32_t *threads) {
   *smem = 0;
   *threads = kThreads;
   switch (variant) {
     case GSB_VARIANT_DIRECT:
-      switch (direct_flavor()) {
-#define GSB_DIRECT_CASE(F)                                                                   \
-  case F:                                                                                    \
-    if (op == GSB_OP_FILL) return probe_direct<GSB_OP_FILL, kDirectU, F>;                    \
-    if (op == GSB_OP_VERIFY) return probe_direct<GSB_OP_VERIFY, kDirectU, F>;                \
-    if (op == GSB_OP_VERIFY_REFILL) return probe_direct<GSB_OP_VERIFY_REFILL, kDirectU, F>;  \
-    return nullptr;
-        GSB_DIRECT_CASE(0)
-#if GSB_LAB
-        GSB_DIRECT_CASE(1)
-        GSB_DIRECT_CASE(2)
-        GSB_DIRECT_CASE(3)
-#endif
-#undef GSB_DIRECT_CASE
-      }
-      return nullptr;
+      return by_op(op, probe_direct<GSB_OP_FILL, kDirectU>, probe_direct<GSB_OP_VERIFY, kDirectU>,
+                   probe_direct<GSB_OP_VERIFY_REFILL, kDirectU>);
     case GSB_VARIANT_CPASYNC:
       // FILL issues no loads, so there is nothing to stage: it takes the direct store path
-      if (op == GSB_OP_FILL) return probe_direct<GSB_OP_FILL, kDirectU, 0>;
-      *smem = kCpSmem;
-      if (op == GSB_OP_VERIFY) return probe_cpasync<GSB_OP_VERIFY, kCpU, kCpS>;
-      if (op == GSB_OP_VERIFY_REFILL) return probe_cpasync<GSB_OP_VERIFY_REFILL, kCpU, kCpS>;
-      return nullptr;
+      if (op != GSB_OP_FILL) *smem = kCpSmem;
+      return by_op(op, probe_direct<GSB_OP_FILL, kDirectU>, probe_cpasync<GSB_OP_VERIFY, kCpU, kCpS>,
+                   probe_cpasync<GSB_OP_VERIFY_REFILL, kCpU, kCpS>);
     case GSB_VARIANT_BULK:
-      // shipped default: 32 KiB tiles x 3 stages, 2 CTAs/SM (96 KiB each of an H100 SM's 228 KiB); on an H100 every
-      // other shape of the lab sweep is within ~1 % of it for every op (DESIGN.md §5)
-      switch (bulk_cfg() >= 0 ? bulk_cfg() : ((GSB_LAB && op == GSB_OP_FILL) ? 5 : 1)) {
-#define GSB_BULK_CASE(ID, U, S)                                                              \
-  case ID:                                                                                   \
-    *smem = U * kThreads * 16 * S;                                                           \
-    if (op == GSB_OP_FILL) return probe_bulk<GSB_OP_FILL, U, S>;                             \
-    if (op == GSB_OP_VERIFY) return probe_bulk<GSB_OP_VERIFY, U, S>;                         \
-    if (op == GSB_OP_VERIFY_REFILL) return probe_bulk<GSB_OP_VERIFY_REFILL, U, S>;           \
-    return nullptr;
-        GSB_BULK_CASE(1, 8, 3)            // 32 KiB x 3 = 96 KiB (2 CTAs/SM)   <- shipped
-#if GSB_LAB
-        GSB_BULK_CASE(0, kBulkU, kBulkS)  // 16 KiB x 4 stages = 64 KiB/CTA (3 CTAs/SM)
-        GSB_BULK_CASE(2, 4, 6)            // 16 KiB x 6 = 96 KiB (2 CTAs/SM)
-        GSB_BULK_CASE(3, 2, 8)            //  8 KiB x 8 = 64 KiB (3 CTAs/SM)
-        GSB_BULK_CASE(4, 4, 3)            // 16 KiB x 3 = 48 KiB (4 CTAs/SM)
-        GSB_BULK_CASE(5, 8, 6)            // 32 KiB x 6 = 192 KiB (1 CTA/SM)
-        GSB_BULK_CASE(6, 16, 3)           // 64 KiB x 3 = 192 KiB (1 CTA/SM)
-        GSB_BULK_CASE(7, 16, 2)           // 64 KiB x 2 = 128 KiB (1 CTA/SM)
-        GSB_BULK_CASE(8, 8, 4)            // 32 KiB x 4 = 128 KiB (1 CTA/SM)
-#endif
-#undef GSB_BULK_CASE
-      }
-      return nullptr;
+      *smem = kBulkSmem;
+      return by_op(op, probe_bulk<GSB_OP_FILL, kBulkU, kBulkS>, probe_bulk<GSB_OP_VERIFY, kBulkU, kBulkS>,
+                   probe_bulk<GSB_OP_VERIFY_REFILL, kBulkU, kBulkS>);
     case GSB_VARIANT_BULKD:
-      // dynamic schedule for the loading ops; FILL keeps the static BULK kernel (32 KiB x 6, 1 CTA/SM)
-#if GSB_LAB
-      if (op == GSB_OP_FILL && !dyn_fill()) {
-        *smem = 8 * kThreads * 16 * 6;
-        return probe_bulk<GSB_OP_FILL, 8, 6>;
-      }
-#endif
-      switch (bulk_cfg() >= 0 ? bulk_cfg() : 1) {  // 32 KiB x 3, 2 CTAs/SM for all three ops
-#define GSB_BULKD_CASE(ID, U, S)                                                             \
-  case ID:                                                                                   \
-    *smem = U * kThreads * 16 * S;                                                           \
-    if (op == GSB_OP_FILL) return probe_bulk_dyn<GSB_OP_FILL, U, S>;                         \
-    if (op == GSB_OP_VERIFY) return probe_bulk_dyn<GSB_OP_VERIFY, U, S>;                     \
-    return probe_bulk_dyn<GSB_OP_VERIFY_REFILL, U, S>;
-        GSB_BULKD_CASE(1, 8, 3)  // <- shipped
-#if GSB_LAB
-        GSB_BULKD_CASE(0, 4, 4)
-        GSB_BULKD_CASE(2, 4, 6)
-        GSB_BULKD_CASE(3, 2, 8)
-        GSB_BULKD_CASE(4, 4, 3)
-        GSB_BULKD_CASE(5, 8, 6)
-        GSB_BULKD_CASE(6, 16, 3)  // 64 KiB x 3 = 192 KiB (1 CTA/SM)
-        GSB_BULKD_CASE(7, 16, 2)  // 64 KiB x 2 = 128 KiB (1 CTA/SM)
-        GSB_BULKD_CASE(8, 8, 4)   // 32 KiB x 4 = 128 KiB (1 CTA/SM)
-#endif
-#undef GSB_BULKD_CASE
-      }
-      return nullptr;
+      *smem = kBulkSmem;
+      return by_op(op, probe_bulk_dyn<GSB_OP_FILL, kBulkU, kBulkS>, probe_bulk_dyn<GSB_OP_VERIFY, kBulkU, kBulkS>,
+                   probe_bulk_dyn<GSB_OP_VERIFY_REFILL, kBulkU, kBulkS>);
     case GSB_VARIANT_BULKW:
-      switch (bulkw_cfg()) {
-#define GSB_BULKW_CASE(ID, WPL, S, WARPS)                                                    \
-  case ID:                                                                                   \
-    *smem = WPL * 512 * S * WARPS;                                                           \
-    *threads = WARPS * 32;                                                                   \
-    if (op == GSB_OP_FILL) return probe_bulk_warp<GSB_OP_FILL, WPL, S, WARPS>;               \
-    if (op == GSB_OP_VERIFY) return probe_bulk_warp<GSB_OP_VERIFY, WPL, S, WARPS>;           \
-    if (op == GSB_OP_VERIFY_REFILL) return probe_bulk_warp<GSB_OP_VERIFY_REFILL, WPL, S, WARPS>; \
-    return nullptr;
-        GSB_BULKW_CASE(0, 8, 3, 8)    //  4 KiB x 3 x 8 warps =  96 KiB/CTA (2 CTAs/SM, 16 warps/SM)
-#if GSB_LAB
-        GSB_BULKW_CASE(1, 8, 6, 4)    //  4 KiB x 6 x 4 warps =  96 KiB     (2 CTAs/SM,  8 warps/SM)
-        GSB_BULKW_CASE(2, 16, 3, 4)   //  8 KiB x 3 x 4 warps =  96 KiB     (2 CTAs/SM,  8 warps/SM)
-        GSB_BULKW_CASE(3, 4, 6, 8)    //  2 KiB x 6 x 8 warps =  96 KiB     (2 CTAs/SM, 16 warps/SM)
-        GSB_BULKW_CASE(4, 8, 4, 4)    //  4 KiB x 4 x 4 warps =  64 KiB     (3 CTAs/SM, 12 warps/SM)
-        GSB_BULKW_CASE(5, 16, 3, 8)   //  8 KiB x 3 x 8 warps = 192 KiB     (1 CTA/SM,   8 warps/SM)
-        GSB_BULKW_CASE(6, 8, 3, 16)   //  4 KiB x 3 x 16 warps = 192 KiB    (1 CTA/SM,  16 warps/SM)
-        GSB_BULKW_CASE(7, 8, 2, 8)    //  4 KiB x 2 x 8 warps =  64 KiB     (3 CTAs/SM, 24 warps/SM)
-#endif
-#undef GSB_BULKW_CASE
-      }
-      return nullptr;
+      *smem = kBulkwSmem;
+      *threads = kBulkwWarps * 32;
+      return by_op(op, probe_bulk_warp<GSB_OP_FILL, kBulkwWpl, kBulkwS, kBulkwWarps>,
+                   probe_bulk_warp<GSB_OP_VERIFY, kBulkwWpl, kBulkwS, kBulkwWarps>,
+                   probe_bulk_warp<GSB_OP_VERIFY_REFILL, kBulkwWpl, kBulkwS, kBulkwWarps>);
     default:
       return nullptr;
   }
@@ -1104,7 +868,6 @@ int gsb_kernel_launch(uint32_t op, const gsb_launch_geom *geom, const gsb_kernel
   probe_fn fn = pick(op, geom->variant, &smem, &threads);
   if (!fn) return (int)cudaErrorInvalidValue;
   gsb_kernel_args a = *args;
-  a.l2_hint = l2_hint_knob();
   a.opaque_zero = 0u;
   fn<<<geom->grid, threads, smem, stream>>>(a);
   return (int)cudaGetLastError();

@@ -49,9 +49,8 @@ if [ "$MODE" = node ]; then
   exit 0
 fi
 if [ "$MODE" = lab ]; then
-  # kernel lab work (needs ./build.sh lab and build/direct_anomaly, both built on the builder and shipped)
+  # kernel lab work (needs build/direct_anomaly, built on the builder and shipped)
   timeout 120 build/direct_anomaly > $OUT/direct_anomaly.json 2> $OUT/direct_anomaly.err
-  timeout 600 python tools/sweep_r02.py > $OUT/sweep_r02.log 2>&1; cp gpurun_out/sweep_r02.json $OUT/ 2>/dev/null
   # one full capture of the shipped refill kernel on a 1 GiB window (profiles/ncu_window_r02_*), and of the shipped VERIFY
   timeout 600 ncu --set full --clock-control none --import-source on -k regex:probe_bulk_dyn -c 2 -o $OUT/ncu_window_dyn_r02 \
     python tools/profile_target.py 5 4 > $OUT/ncu_full.log 2>&1
@@ -60,7 +59,7 @@ if [ "$MODE" = lab ]; then
   ncu -i $OUT/ncu_transient_r02.ncu-rep --page raw --csv > $OUT/ncu_transient_r02_raw.csv 2>/dev/null
   ncu -i $OUT/ncu_window_dyn_r02.ncu-rep --page raw --csv > $OUT/ncu_window_dyn_r02_raw.csv 2>/dev/null
   ncu -i $OUT/ncu_window_dyn_r02.ncu-rep --page details --csv > $OUT/ncu_window_dyn_r02_details.csv 2>/dev/null
-  tail -5 $OUT/sweep_r02.log
+  tail -c 300 $OUT/direct_anomaly.json
   exit 0
 fi
 timeout 900 python -m pytest tests -m gpu -x -q -rs > $OUT/pytest_gpu.log 2>&1; echo "pytest rc=$?" >> $OUT/pytest_gpu.log
@@ -77,8 +76,8 @@ timeout 400 python bench.py --steps 200 --warmup 5 --quick-allocate > $OUT/bench
 # launch list of the same command (shares, not absolutes: ncu serialises and runs cold)
 timeout 600 ncu --metrics gpu__time_duration.sum --clock-control none -c 400 --csv --log-file $OUT/launches.csv \
   python bench.py --steps 20 --warmup 3 --no-allocate --no-cpu-baseline > $OUT/bench_under_ncu.log 2>&1
-# the DIRECT control after its refill fix (lab library: same source, all shapes)
-SWEEP_ONLY=direct timeout 200 python tools/sweep_r02.py > $OUT/sweep_direct.log 2>&1; cp gpurun_out/sweep_r02_direct.json $OUT/ 2>/dev/null
+# the DIRECT control: the same headline on the unstaged load -> store path
+timeout 400 python bench.py --variant direct --steps 20 --warmup 5 --no-allocate --no-cpu-baseline > $OUT/bench_direct.json 2> $OUT/bench_direct.err
 # memcheck + racecheck of every data path on a small arena (the smoke), this round's kernels
 GSB_PROBE_WATCHDOG_MS=0 timeout 600 compute-sanitizer --tool memcheck --error-exitcode 3 python __graft_entry__.py smoke-only > $OUT/memcheck_smoke.log 2>&1; echo "memcheck rc=$?" >> $OUT/memcheck_smoke.log
 GSB_PROBE_WATCHDOG_MS=0 timeout 600 compute-sanitizer --tool racecheck --error-exitcode 3 python tools/profile_target.py 5 2 > $OUT/racecheck_bulkd.log 2>&1; echo "racecheck rc=$?" >> $OUT/racecheck_bulkd.log
