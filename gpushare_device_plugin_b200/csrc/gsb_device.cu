@@ -159,7 +159,7 @@ struct Device {
   gsb_kernel_out *out_host = nullptr, *out_dev = nullptr;
   gsb_partial *partials = nullptr;
   unsigned int *ticket = nullptr;
-  unsigned long long *tile_counter = nullptr;
+  unsigned long long *tile_counter = nullptr;  // [2]: BULKD tile claims, verify tiles a refill has consumed
   uint32_t *seed_table = nullptr;  // generation that last wrote each granule (written only by the kernels' last CTA)
   uint32_t launch_seq = 0;
   gsb_fault_log *fault_log = nullptr;                                // device memory: the kernels' fault log
@@ -366,8 +366,8 @@ int ensure_ready(Device *d) {
                     sizeof(gsb_partial) * gsb_kernel_max_grid((int)d->sm_count)));
   RT_TRY(cudaMalloc(reinterpret_cast<void **>(&d->ticket), sizeof(unsigned int)));
   RT_TRY(cudaMemset(d->ticket, 0, sizeof(unsigned int)));
-  RT_TRY(cudaMalloc(reinterpret_cast<void **>(&d->tile_counter), sizeof(unsigned long long)));
-  RT_TRY(cudaMemset(d->tile_counter, 0, sizeof(unsigned long long)));
+  RT_TRY(cudaMalloc(reinterpret_cast<void **>(&d->tile_counter), 2 * sizeof(unsigned long long)));
+  RT_TRY(cudaMemset(d->tile_counter, 0, 2 * sizeof(unsigned long long)));
   RT_TRY(cudaMalloc(reinterpret_cast<void **>(&d->fault_log), sizeof(gsb_fault_log)));
   RT_TRY(cudaMemset(d->fault_log, 0, sizeof(gsb_fault_log)));
   RT_TRY(cudaHostAlloc(reinterpret_cast<void **>(&d->fault_host), sizeof(gsb_fault_log),

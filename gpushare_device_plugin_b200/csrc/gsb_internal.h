@@ -60,7 +60,9 @@ struct gsb_kernel_args {
   uint32_t opaque_zero;        /* always 0; only the compiler does not know (DIRECT refill: a real load->store dependency) */
   gsb_partial *partials;       /* [grid] device memory */
   unsigned int *ticket;        /* device memory, self-resetting */
-  unsigned long long *tile_counter; /* device memory, self-resetting: dynamic tile scheduler of BULKD */
+  /* device memory, self-resetting, two counters of BULKD: [0] the dynamic tile scheduler's claims, [1] the verify
+   * tiles a refill has consumed */
+  unsigned long long *tile_counter;
   gsb_kernel_out *out;         /* device pointer of the mapped host struct */
   gsb_fault_log *fault;        /* device memory, self-resetting (zero between faulted launches) */
   gsb_fault_log *fault_out;    /* device pointer of the mapped host copy */

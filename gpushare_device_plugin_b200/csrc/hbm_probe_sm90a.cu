@@ -18,7 +18,9 @@
  * Kernels: the two GSB_VARIANT_AUTO launches — BULKD (FILL, VERIFY_REFILL) and BULK (VERIFY), one TMA ring with two
  * tile schedules, 32 KiB x 3 stages — plus one shape each of DIRECT, CPASYNC and BULKW, kept as independent data
  * paths for the parity tests (five implementations, one answer). Every shape is fixed at compile time; the H100
- * tile-shape sweep behind the BULK / BULKD shape is in DESIGN.md §5.
+ * tile-shape sweep behind the BULK / BULKD shape is in DESIGN.md §5. The BULKD refill runs as a verify pass over the
+ * whole window and then a write pass, in one launch (HBM serves that faster than reads and writes to the same rows at
+ * once); the other refills walk the window in place, each tile loaded and then stored.
  *
  * Reduction: per-thread registers -> warp shuffles -> one gsb_partial slot per CTA (plain stores,
  * no atomics on the data path) -> a self-resetting ticket elects the last CTA, which folds all
@@ -133,6 +135,11 @@ __device__ __forceinline__ void bulk_wait_all() {
 }
 __device__ __forceinline__ void fence_proxy_async_smem() {
   asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
+}
+__device__ __forceinline__ unsigned long long globaltimer() {
+  unsigned long long t;
+  asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t));
+  return t;
 }
 
 // ---------------------------------------------------------------- pattern + compare
@@ -378,7 +385,7 @@ __device__ void finish(const gsb_kernel_args &a, const Acc &acc) {
   }
   if (threadIdx.x == 0) {
     *a.ticket = 0u;  // self-reset: the next launch on this stream starts from 0
-    if (a.tile_counter) *a.tile_counter = 0ull;
+    if (a.tile_counter) a.tile_counter[0] = a.tile_counter[1] = 0ull;  // every other CTA is past the refill's gate
     gsb_kernel_out *o = a.out;
     o->mismatch_words = all.mismatch_words;
     o->mismatch_bits = all.mismatch_bits;
@@ -497,9 +504,12 @@ __global__ void __launch_bounds__(kThreads) probe_cpasync(const gsb_kernel_args 
 //   next(k, s)  leader, once per slot in slot order: the tile slot k (stage s) holds, or the end of the walk
 //   tile(k, s)  every thread, after slot k's barrier: the same tile
 //   done(t)     t is the end of the walk
+//   kPasses     1: every slot does OP to its tile; 2 (refill only): a slot tile t < n_tiles is verified, and
+//               n_tiles + t writes tile t (the refill's two passes, below)
 
 // BULK: slot k holds tile blockIdx + k * grid while k < my_n; every thread computes it.
 struct StaticSchedule {
+  static constexpr int kPasses = 1;
   unsigned long long my_n;
   __device__ StaticSchedule(const gsb_kernel_args &, unsigned long long n_tiles, unsigned long long *)
       : my_n(n_tiles > blockIdx.x ? (n_tiles - blockIdx.x + gridDim.x - 1) / gridDim.x : 0ull) {}
@@ -513,13 +523,16 @@ struct StaticSchedule {
 // take more tiles and the kernel ends with every CTA busy (no straggler tail). Claims are made in time order, so
 // concurrently processed tiles stay neighbours in memory. The claimed index travels to the consumers through
 // tile_of[s] under the stage's mbarrier (arrive = release, wait = acquire); every slot is issued, and the first one
-// past the last tile holds kDone.
+// past the last claim holds kDone. With two passes the counter runs over 2 * n_tiles claims, so claims are monotone:
+// inside one CTA every slot of the verify pass comes before every slot of the write pass.
+template <int PASSES>
 struct ClaimedSchedule {
+  static constexpr int kPasses = PASSES;
   static constexpr unsigned long long kDone = ~0ull;
-  unsigned long long n_tiles, in_hand = 0;
+  unsigned long long n_claims, in_hand = 0;
   unsigned long long *counter, *tile_of;
   __device__ ClaimedSchedule(const gsb_kernel_args &a, unsigned long long n, unsigned long long *slots)
-      : n_tiles(n), counter(a.tile_counter), tile_of(slots) {
+      : n_claims(PASSES * n), counter(a.tile_counter), tile_of(slots) {
     // the leader always holds one claim in hand: the atomic for the NEXT tile is issued when the current one is
     // consumed, so its ~L2 round trip overlaps the tile being processed instead of delaying the next load
     if (threadIdx.x == 0) in_hand = atomicAdd(counter, 1ull);
@@ -528,24 +541,60 @@ struct ClaimedSchedule {
   __device__ unsigned long long next(unsigned long long, int s) {
     const unsigned long long t = in_hand;
     in_hand = atomicAdd(counter, 1ull);
-    return tile_of[s] = t < n_tiles ? t : kDone;
+    return tile_of[s] = t < n_claims ? t : kDone;
   }
   __device__ unsigned long long tile(unsigned long long, int s) const { return tile_of[s]; }
   __device__ static bool done(unsigned long long t) { return t == kDone; }
 };
 
+// The refill's two passes. A refill stores the next generation's pattern, which depends on the address and the seed
+// only, so the window can be verified completely and then written completely: same memory image, same results, same
+// 2 * W bytes. HBM serves a read pass and a write pass faster than it serves reads and writes to the same rows at
+// once (DESIGN.md §5). One rule keeps it correct: the store of tile t must not reach HBM while another CTA's bulk load
+// of tile t may still be reading it. So each CTA adds the verify tiles it has consumed (past their mbarrier) to the
+// launch's count, tile_counter[1], once, when it leaves the verify pass: at its first write slot or at the end of the
+// walk. A CTA with tiles to write then waits, before it writes any, until the count reaches n_tiles; it waits when it
+// consumes its first write slot, never when its leader claims or issues one, since the leader is a consumer too. This
+// cannot deadlock whatever the residency: verify tiles are claimed only by running CTAs, and such a CTA waits on
+// nothing but its own loads until it has added its count. The wait is bounded: a CTA that has waited kGateTimeoutNs
+// drops its write tiles, so words_done falls short of n_words and the host reports the launch as failed instead of
+// the GPU spinning for ever.
+constexpr unsigned long long kGateTimeoutNs = 1000000000ull;
+
+// leader, once per CTA; false: the gate did not open in time
+__device__ __forceinline__ bool leave_verify_pass(unsigned long long *verified, unsigned long long mine,
+                                                  unsigned long long n_tiles, bool will_write) {
+  asm volatile("red.release.gpu.global.add.u64 [%0], %1;" ::"l"(verified), "l"(mine) : "memory");
+  if (!will_write) return true;
+  const unsigned long long t0 = globaltimer();
+  for (;;) {
+    unsigned long long seen;
+    asm volatile("ld.acquire.gpu.global.u64 %0, [%1];" : "=l"(seen) : "l"(verified) : "memory");
+    if (seen >= n_tiles) break;
+    if (globaltimer() - t0 > kGateTimeoutNs) return false;
+    __nanosleep(64);
+  }
+  asm volatile("fence.proxy.async.global;" ::: "memory");  // the bulk stores that follow come after the acquire
+  return true;
+}
+
 template <int OP, int U, int S, typename Schedule>
 __device__ __forceinline__ void bulk_ring(const gsb_kernel_args &a) {
+  constexpr bool kTwoPass = Schedule::kPasses == 2;
+  static_assert(!kTwoPass || OP == GSB_OP_VERIFY_REFILL, "only a refill runs as a verify pass and a write pass");
   constexpr unsigned long long TILE = (unsigned long long)kThreads * U;
   extern __shared__ __align__(128) unsigned char smem_raw[];
   uint4 *ring = reinterpret_cast<uint4 *>(smem_raw);  // [S][TILE]
   __shared__ __align__(8) unsigned long long full_bar[S];
   __shared__ unsigned long long tile_of[S];  // ClaimedSchedule only
+  __shared__ int gate_open;                  // two passes: this CTA may write its write-pass tiles
   const unsigned long long n_tiles = (a.n_words + TILE - 1) / TILE;
   Schedule sched(a, n_tiles, tile_of);
   const uint32_t key_write = gsb_seed_key(a.seed_write);
   uint4 *__restrict__ win = a.base + a.first_word;
   const bool leader = threadIdx.x == 0;
+  unsigned long long verified = 0;  // two passes, leader: verify-pass slots this CTA has consumed
+  bool verifying = true;            // two passes, leader: this CTA has not yet left the verify pass
   Acc acc;
 
   auto words_of = [&](unsigned long long t) -> uint32_t {
@@ -556,8 +605,9 @@ __device__ __forceinline__ void bulk_ring(const gsb_kernel_args &a) {
     if (!sched.has(k)) return;
     const int s = (int)(k % S);
     const unsigned long long t = sched.next(k, s);
-    if (Schedule::done(t)) {
-      mbar_arrive(smem_u32(&full_bar[s]));  // no tile: the consumers still pass the barrier, and read kDone
+    if (Schedule::done(t) || (kTwoPass && t >= n_tiles)) {
+      // nothing to load (end of the walk, or a write-pass tile): the consumers still pass the barrier and read the slot
+      mbar_arrive(smem_u32(&full_bar[s]));
       return;
     }
     const uint32_t bytes = words_of(t) * 16u;
@@ -570,12 +620,13 @@ __device__ __forceinline__ void bulk_ring(const gsb_kernel_args &a) {
 #pragma unroll
     for (int s = 0; s < S; s++) mbar_init(smem_u32(&full_bar[s]), 1u);
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
+    gate_open = 1;
   }
   __syncthreads();
 
-  // prologue: VERIFY can keep all S stages in flight (a consumed stage is refilled at once);
-  // VERIFY_REFILL keeps S-1 (a stage is refilled one iteration after its store was issued)
-  constexpr int kPrologue = (OP == GSB_OP_VERIFY) ? S : S - 1;
+  // prologue: VERIFY and the two-pass refill can keep all S stages in flight (a consumed stage is reloaded at once);
+  // the in-place VERIFY_REFILL keeps S-1 (a stage is reloaded one iteration after its store was issued)
+  constexpr int kPrologue = (OP == GSB_OP_VERIFY || kTwoPass) ? S : S - 1;
   if (OP != GSB_OP_FILL && leader)
     for (int k = 0; k < kPrologue; k++) load(k);
 
@@ -590,25 +641,72 @@ __device__ __forceinline__ void bulk_ring(const gsb_kernel_args &a) {
     } else {
       mbar_wait(smem_u32(&full_bar[s]), (uint32_t)((k / S) & 1ull));
     }
-    const unsigned long long t = sched.tile(k, s);
-    if (Schedule::done(t)) break;  // uniform: every thread reads the same slot after the same barrier
-    const uint32_t nw_tile = words_of(t);
-    uint4 *stage = ring + s * TILE;
-    const uint32_t key_expect = (OP != GSB_OP_FILL) ? expect_key_of(a, a.first_word + t * TILE) : 0u;
-#pragma unroll
-    for (int u = 0; u < U; u++) {
-      const uint32_t i = u * kThreads + threadIdx.x;
-      if (i < nw_tile) {
-        uint4 v = make_uint4(0, 0, 0, 0);
-        if (OP != GSB_OP_FILL) v = stage[i];
-        const uint4 nw = process_word<OP>(a, v, a.first_word + t * TILE + i, key_expect, key_write, acc);
-        if (OP != GSB_OP_VERIFY) stage[i] = nw;
+    unsigned long long t = sched.tile(k, s);
+    bool reads = OP != GSB_OP_FILL;  // two passes: a verify-pass slot reads and compares, a write-pass slot writes
+    if (kTwoPass) {
+      if (Schedule::done(t) || t >= n_tiles) {
+        if (leader) {
+          if (verifying) {
+            verifying = false;
+            gate_open = leave_verify_pass(a.tile_counter + 1, verified, n_tiles, !Schedule::done(t));
+          }
+          bulk_wait_read<S - 1>();  // the bulk store that last read this stage (slot k-S) has drained it
+        }
+        __syncthreads();
+        if (!gate_open) break;  // uniform; only the leader writes gate_open, and only before this barrier
+        if (!Schedule::done(t)) t -= n_tiles;
+        reads = false;
+      } else if (leader) {
+        verified += 1;
       }
     }
-    if (OP != GSB_OP_VERIFY) fence_proxy_async_smem();  // generic-proxy writes -> visible to the bulk engine
+    if (Schedule::done(t)) break;  // uniform: every thread reads the same slot after the same barrier
+    const bool writes = kTwoPass ? !reads : OP != GSB_OP_VERIFY;
+    const uint32_t nw_tile = words_of(t);
+    uint4 *stage = ring + s * TILE;
+    const uint32_t key_expect = reads ? expect_key_of(a, a.first_word + t * TILE) : 0u;
+    if (kTwoPass && reads) {  // compare and fold what was read; its words are counted when they are written
+#pragma unroll
+      for (int u = 0; u < U; u++) {
+        const uint32_t i = u * kThreads + threadIdx.x;
+        if (i < nw_tile) {
+          const unsigned long long w = a.first_word + t * TILE + i;
+          const uint4 v = stage[i];
+          fold_checksum(v, acc);
+          compare_word(v, pattern_from_key(gsb_word_key(w), key_expect), w, acc, a.fault);
+        }
+      }
+    } else if (kTwoPass) {  // the next generation; folds nothing (the checksums are of the words read)
+#pragma unroll
+      for (int u = 0; u < U; u++) {
+        const uint32_t i = u * kThreads + threadIdx.x;
+        if (i < nw_tile) {
+          stage[i] = pattern_from_key(gsb_word_key(a.first_word + t * TILE + i), key_write);
+          acc.words += 1u;
+        }
+      }
+    } else {
+#pragma unroll
+      for (int u = 0; u < U; u++) {
+        const uint32_t i = u * kThreads + threadIdx.x;
+        if (i < nw_tile) {
+          uint4 v = make_uint4(0, 0, 0, 0);
+          if (OP != GSB_OP_FILL) v = stage[i];
+          const uint4 nw = process_word<OP>(a, v, a.first_word + t * TILE + i, key_expect, key_write, acc);
+          if (OP != GSB_OP_VERIFY) stage[i] = nw;
+        }
+      }
+    }
+    if (writes) fence_proxy_async_smem();  // generic-proxy writes -> visible to the bulk engine
     __syncthreads();  // every thread is done with this stage (reads, and writes + proxy fence)
     if (leader) {
-      if (OP == GSB_OP_VERIFY) {
+      if (kTwoPass) {
+        if (writes) {
+          bulk_s2g(win + t * TILE, smem_u32(stage), nw_tile * 16u);
+          bulk_commit();
+        }
+        load(k + S);  // same stage: a load once the barrier has released it, or (write pass) only the claim
+      } else if (OP == GSB_OP_VERIFY) {
         load(k + S);  // same stage, just released by the barrier
       } else {
         bulk_s2g(win + t * TILE, smem_u32(stage), nw_tile * 16u);
@@ -633,7 +731,7 @@ __global__ void __launch_bounds__(kThreads) probe_bulk(const gsb_kernel_args a) 
 
 template <int OP, int U, int S>
 __global__ void __launch_bounds__(kThreads) probe_bulk_dyn(const gsb_kernel_args a) {
-  bulk_ring<OP, U, S, ClaimedSchedule>(a);
+  bulk_ring<OP, U, S, ClaimedSchedule<OP == GSB_OP_VERIFY_REFILL ? 2 : 1>>(a);
 }
 
 // ---------------------------------------------------------------- BULKW (per-warp TMA rings)
@@ -808,12 +906,10 @@ probe_fn pick(uint32_t op, uint32_t variant, uint32_t *smem, uint32_t *threads) 
 
 // test hook (gsb_test_stall): hold the stream for `ns` nanoseconds
 __global__ void stall_kernel(unsigned long long ns) {
-  unsigned long long t0, t;
-  asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t0));
+  const unsigned long long t0 = globaltimer();
   do {
     __nanosleep(1000);
-    asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t));
-  } while (t - t0 < ns);
+  } while (globaltimer() - t0 < ns);
 }
 
 }  // namespace
