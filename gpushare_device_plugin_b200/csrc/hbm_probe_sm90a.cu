@@ -15,12 +15,13 @@
  *            st.shared.v4 -> cp.async.bulk shared->global
  * All are persistent kernels over fixed-size tiles, grid = resident CTAs/SM x #SMs.
  *
- * Kernels: the two GSB_VARIANT_AUTO launches — BULKD (FILL, VERIFY_REFILL) and BULK (VERIFY), one TMA ring with two
- * tile schedules, 32 KiB x 3 stages — plus one shape each of DIRECT, CPASYNC and BULKW, kept as independent data
- * paths for the parity tests (five implementations, one answer). Every shape is fixed at compile time; the H100
- * tile-shape sweep behind the BULK / BULKD shape is in DESIGN.md §5. The BULKD refill runs as a verify pass over the
- * whole window and then a write pass, in one launch (HBM serves that faster than reads and writes to the same rows at
- * once); the other refills walk the window in place, each tile loaded and then stored.
+ * Kernels: the two GSB_VARIANT_AUTO launches — BULKD (FILL, VERIFY_REFILL) and BULK (VERIFY), 32 KiB x 3 stages —
+ * plus one shape each of DIRECT, CPASYNC and BULKW, kept as independent data paths for the parity tests (five
+ * implementations, one answer). BULK, BULKD and BULKW run one TMA ring protocol (bulk_ring): one ring per CTA with a
+ * static or a claimed tile schedule, or, for BULKW, one ring per warp with the static schedule. Every shape is fixed
+ * at compile time; the H100 tile-shape sweep behind the BULK / BULKD shape is in DESIGN.md §5. The BULKD refill runs
+ * as a verify pass over the whole window and then a write pass, in one launch (HBM serves that faster than reads and
+ * writes to the same rows at once); the other refills walk the window in place, each tile loaded and then stored.
  *
  * Reduction: per-thread registers -> warp shuffles -> one gsb_partial slot per CTA (plain stores,
  * no atomics on the data path) -> a self-resetting ticket elects the last CTA, which folds all
@@ -229,22 +230,34 @@ __device__ __forceinline__ uint32_t expect_key_of(const gsb_kernel_args &a, unsi
   return gsb_seed_key(s);
 }
 
-// one word: OP is a compile-time GSB_OP_*; `v` is the loaded value (ignored for FILL); returns the
-// value to store (undefined for VERIFY)
-template <int OP>
+// What is done to one word, as compile-time flags:
+//   kRead         `v` is the loaded word: fold it into the checksums and compare it with the expected pattern
+//   kWrite        return the next generation's word (otherwise the return value is undefined)
+//   kFoldWritten  fold the returned word into the checksums (FILL, which reads nothing)
+//   kCount        count the word in words_done
+constexpr unsigned kRead = 1u, kWrite = 2u, kFoldWritten = 4u, kCount = 8u;
+
+// the flags of a launch that does OP (a compile-time GSB_OP_*) to every word once
+__host__ __device__ constexpr unsigned op_words(int op) {
+  return op == GSB_OP_FILL     ? kWrite | kFoldWritten | kCount
+         : op == GSB_OP_VERIFY ? kRead | kCount
+                               : kRead | kWrite | kCount;
+}
+
+template <unsigned F>
 __device__ __forceinline__ uint4 process_word(const gsb_kernel_args &a, const uint4 v, unsigned long long w,
                                               uint32_t key_expect, uint32_t key_write, Acc &acc) {
   const uint32_t m = gsb_word_key(w);
   uint4 nw = make_uint4(0, 0, 0, 0);
-  if (OP != GSB_OP_FILL) {
+  if (F & kRead) {
     fold_checksum(v, acc);
     compare_word(v, pattern_from_key(m, key_expect), w, acc, a.fault);
   }
-  if (OP != GSB_OP_VERIFY) {
+  if (F & kWrite) {
     nw = pattern_from_key(m, key_write);
-    if (OP == GSB_OP_FILL) fold_checksum(nw, acc);
+    if (F & kFoldWritten) fold_checksum(nw, acc);
   }
-  acc.words += 1u;
+  if (F & kCount) acc.words += 1u;
   return nw;
 }
 
@@ -421,7 +434,7 @@ __global__ void __launch_bounds__(kThreads) probe_direct(const gsb_kernel_args a
 #pragma unroll
       for (int u = 0; u < U; u++) {
         const unsigned long long l = l0 + (unsigned long long)u * kThreads;
-        uint4 nw = process_word<OP>(a, v[u], a.first_word + l, key_expect, key_write, acc);
+        uint4 nw = process_word<op_words(OP)>(a, v[u], a.first_word + l, key_expect, key_write, acc);
         if (OP == GSB_OP_VERIFY_REFILL) nw = after_load(nw, v[u].x ^ v[u].y ^ v[u].z ^ v[u].w, a.opaque_zero);
         if (OP != GSB_OP_VERIFY) st_stream(win + l, nw);
       }
@@ -431,7 +444,7 @@ __global__ void __launch_bounds__(kThreads) probe_direct(const gsb_kernel_args a
         const unsigned long long l = l0 + (unsigned long long)u * kThreads;
         if (l < a.n_words) {
           if (OP != GSB_OP_FILL) v[u] = ld_stream(win + l);
-          uint4 nw = process_word<OP>(a, v[u], a.first_word + l, key_expect, key_write, acc);
+          uint4 nw = process_word<op_words(OP)>(a, v[u], a.first_word + l, key_expect, key_write, acc);
           if (OP == GSB_OP_VERIFY_REFILL) nw = after_load(nw, v[u].x ^ v[u].y ^ v[u].z ^ v[u].w, a.opaque_zero);
           if (OP != GSB_OP_VERIFY) st_stream(win + l, nw);
         }
@@ -485,7 +498,7 @@ __global__ void __launch_bounds__(kThreads) probe_cpasync(const gsb_kernel_args 
       if (l < a.n_words) {
         // each thread reads back only the slots it copied itself: no CTA barrier needed
         const uint4 v = ring[s * TILE + u * kThreads + threadIdx.x];
-        const uint4 nw = process_word<OP>(a, v, a.first_word + l, key_expect, key_write, acc);
+        const uint4 nw = process_word<op_words(OP)>(a, v, a.first_word + l, key_expect, key_write, acc);
         if (OP != GSB_OP_VERIFY) st_stream(win + l, nw);
       }
     }
@@ -494,28 +507,35 @@ __global__ void __launch_bounds__(kThreads) probe_cpasync(const gsb_kernel_args 
   finish(a, acc);
 }
 
-// ---------------------------------------------------------------- BULK / BULKD (TMA 1-D ring)
+// ---------------------------------------------------------------- BULK / BULKD / BULKW (TMA 1-D rings)
 //
-// One ring of S stages of TILE words. The leader (thread 0) starts the bulk load of slot k into stage k % S and
-// completes it on the stage's mbarrier; all threads process the tile in shared memory; the leader writes it back
-// with a bulk store. Which tile slot k holds is the schedule's business; the schedule is a template argument, so
-// nothing that differs between the two is decided at run time:
+// A CTA runs RINGS rings: one for BULK and BULKD, one per warp for BULKW. Ring r has its own S stages of TILE words
+// and its own mbarriers. Its leader (its first thread) starts the bulk load of slot k into stage k % S and completes
+// it on the stage's mbarrier; the ring's threads process the tile in shared memory; the leader writes it back with a
+// bulk store. A per-warp ring synchronises with __syncwarp only, so a warp waiting on HBM never holds the CTA's other
+// warps at a barrier. Which tile slot k holds is the schedule's business; the schedule is a template argument, so
+// nothing that differs between the two is decided at run time. Each schedule is built with its ring's index:
 //   has(k)      slot k is issued at all: the loop stops before waiting on a slot whose load was never issued
 //   next(k, s)  leader, once per slot in slot order: the tile slot k (stage s) holds, or the end of the walk
-//   tile(k, s)  every thread, after slot k's barrier: the same tile
+//   tile(k, s)  every thread of the ring, after slot k's barrier: the same tile
 //   done(t)     t is the end of the walk
 //   kPasses     1: every slot does OP to its tile; 2 (refill only): a slot tile t < n_tiles is verified, and
 //               n_tiles + t writes tile t (the refill's two passes, below)
 
-// BULK: slot k holds tile blockIdx + k * grid while k < my_n; every thread computes it.
+// BULK (RINGS = 1) and BULKW: ring r's slot k holds tile (blockIdx + k * grid) * RINGS + r while k < my_n, so the rings
+// of a CTA take adjacent tiles, which keeps DRAM pages hot; every thread computes it.
+template <int RINGS>
 struct StaticSchedule {
   static constexpr int kPasses = 1;
-  unsigned long long my_n;
-  __device__ StaticSchedule(const gsb_kernel_args &, unsigned long long n_tiles, unsigned long long *)
-      : my_n(n_tiles > blockIdx.x ? (n_tiles - blockIdx.x + gridDim.x - 1) / gridDim.x : 0ull) {}
+  unsigned long long first, my_n;
+  __device__ StaticSchedule(const gsb_kernel_args &, unsigned long long n_tiles, int r, unsigned long long *)
+      : first((unsigned long long)blockIdx.x * RINGS + r) {
+    const unsigned long long stride = (unsigned long long)gridDim.x * RINGS;
+    my_n = n_tiles > first ? (n_tiles - first + stride - 1) / stride : 0ull;
+  }
   __device__ bool has(unsigned long long k) const { return k < my_n; }
   __device__ unsigned long long next(unsigned long long k, int s) const { return tile(k, s); }
-  __device__ unsigned long long tile(unsigned long long k, int) const { return blockIdx.x + k * gridDim.x; }
+  __device__ unsigned long long tile(unsigned long long k, int) const { return first + k * gridDim.x * RINGS; }
   __device__ static bool done(unsigned long long) { return false; }
 };
 
@@ -524,14 +544,15 @@ struct StaticSchedule {
 // concurrently processed tiles stay neighbours in memory. The claimed index travels to the consumers through
 // tile_of[s] under the stage's mbarrier (arrive = release, wait = acquire); every slot is issued, and the first one
 // past the last claim holds kDone. With two passes the counter runs over 2 * n_tiles claims, so claims are monotone:
-// inside one CTA every slot of the verify pass comes before every slot of the write pass.
+// inside one CTA every slot of the verify pass comes before every slot of the write pass. The schedule is CTA-wide
+// (RINGS = 1): its leader is thread 0, and the ring index is always 0.
 template <int PASSES>
 struct ClaimedSchedule {
   static constexpr int kPasses = PASSES;
   static constexpr unsigned long long kDone = ~0ull;
   unsigned long long n_claims, in_hand = 0;
   unsigned long long *counter, *tile_of;
-  __device__ ClaimedSchedule(const gsb_kernel_args &a, unsigned long long n, unsigned long long *slots)
+  __device__ ClaimedSchedule(const gsb_kernel_args &a, unsigned long long n, int, unsigned long long *slots)
       : n_claims(PASSES * n), counter(a.tile_counter), tile_of(slots) {
     // the leader always holds one claim in hand: the atomic for the NEXT tile is issued when the current one is
     // consumed, so its ~L2 round trip overlaps the tile being processed instead of delaying the next load
@@ -578,21 +599,49 @@ __device__ __forceinline__ bool leave_verify_pass(unsigned long long *verified, 
   return true;
 }
 
-template <int OP, int U, int S, typename Schedule>
+// one ring thread's words of a staged tile: n words from absolute word w0, the thread's words i = u * T + rt;
+// F says what is done to each (process_word)
+template <unsigned F, int U, int T>
+__device__ __forceinline__ void process_stage(const gsb_kernel_args &a, uint4 *stage, unsigned long long w0,
+                                              uint32_t n, uint32_t rt, uint32_t key_expect, uint32_t key_write,
+                                              Acc &acc) {
+#pragma unroll
+  for (int u = 0; u < U; u++) {
+    const uint32_t i = u * T + rt;
+    if (i < n) {
+      uint4 v = make_uint4(0, 0, 0, 0);
+      if (F & kRead) v = stage[i];
+      const uint4 nw = process_word<F>(a, v, w0 + i, key_expect, key_write, acc);
+      if (F & kWrite) stage[i] = nw;
+    }
+  }
+}
+
+// RINGS rings per CTA, each of S stages of U words per ring thread
+template <int OP, int U, int S, int RINGS, typename Schedule>
 __device__ __forceinline__ void bulk_ring(const gsb_kernel_args &a) {
   constexpr bool kTwoPass = Schedule::kPasses == 2;
   static_assert(!kTwoPass || OP == GSB_OP_VERIFY_REFILL, "only a refill runs as a verify pass and a write pass");
-  constexpr unsigned long long TILE = (unsigned long long)kThreads * U;
+  static_assert(RINGS == 1 || (kThreads == RINGS * 32 && !kTwoPass), "one ring per CTA, or one per warp");
+  constexpr int kRingThreads = kThreads / RINGS;
+  constexpr unsigned long long TILE = (unsigned long long)U * kRingThreads;
+  const int r = RINGS == 1 ? 0 : (int)(threadIdx.x / kRingThreads);            // this thread's ring
+  const uint32_t rt = RINGS == 1 ? threadIdx.x : threadIdx.x % kRingThreads;  // its thread in the ring
+  auto ring_sync = [] {
+    if (RINGS == 1) __syncthreads();
+    else __syncwarp();
+  };
   extern __shared__ __align__(128) unsigned char smem_raw[];
-  uint4 *ring = reinterpret_cast<uint4 *>(smem_raw);  // [S][TILE]
-  __shared__ __align__(8) unsigned long long full_bar[S];
+  uint4 *ring = reinterpret_cast<uint4 *>(smem_raw) + r * S * TILE;  // [S][TILE]
+  __shared__ __align__(8) unsigned long long full_bars[RINGS][S];
+  unsigned long long *full_bar = full_bars[r];
   __shared__ unsigned long long tile_of[S];  // ClaimedSchedule only
   __shared__ int gate_open;                  // two passes: this CTA may write its write-pass tiles
   const unsigned long long n_tiles = (a.n_words + TILE - 1) / TILE;
-  Schedule sched(a, n_tiles, tile_of);
+  Schedule sched(a, n_tiles, r, tile_of);
   const uint32_t key_write = gsb_seed_key(a.seed_write);
   uint4 *__restrict__ win = a.base + a.first_word;
-  const bool leader = threadIdx.x == 0;
+  const bool leader = rt == 0;
   unsigned long long verified = 0;  // two passes, leader: verify-pass slots this CTA has consumed
   bool verifying = true;            // two passes, leader: this CTA has not yet left the verify pass
   Acc acc;
@@ -620,9 +669,9 @@ __device__ __forceinline__ void bulk_ring(const gsb_kernel_args &a) {
 #pragma unroll
     for (int s = 0; s < S; s++) mbar_init(smem_u32(&full_bar[s]), 1u);
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-    gate_open = 1;
+    if (kTwoPass) gate_open = 1;
   }
-  __syncthreads();
+  __syncthreads();  // the zeroed fault histogram and every ring's mbarriers
 
   // prologue: VERIFY and the two-pass refill can keep all S stages in flight (a consumed stage is reloaded at once);
   // the in-place VERIFY_REFILL keeps S-1 (a stage is reloaded one iteration after its store was issued)
@@ -637,7 +686,7 @@ __device__ __forceinline__ void bulk_ring(const gsb_kernel_args &a) {
         bulk_wait_read<S - 1>();  // the bulk store that last read this stage (slot k-S) has drained it
         sched.next(k, s);
       }
-      __syncthreads();
+      ring_sync();
     } else {
       mbar_wait(smem_u32(&full_bar[s]), (uint32_t)((k / S) & 1ull));
     }
@@ -664,41 +713,16 @@ __device__ __forceinline__ void bulk_ring(const gsb_kernel_args &a) {
     const bool writes = kTwoPass ? !reads : OP != GSB_OP_VERIFY;
     const uint32_t nw_tile = words_of(t);
     uint4 *stage = ring + s * TILE;
-    const uint32_t key_expect = reads ? expect_key_of(a, a.first_word + t * TILE) : 0u;
-    if (kTwoPass && reads) {  // compare and fold what was read; its words are counted when they are written
-#pragma unroll
-      for (int u = 0; u < U; u++) {
-        const uint32_t i = u * kThreads + threadIdx.x;
-        if (i < nw_tile) {
-          const unsigned long long w = a.first_word + t * TILE + i;
-          const uint4 v = stage[i];
-          fold_checksum(v, acc);
-          compare_word(v, pattern_from_key(gsb_word_key(w), key_expect), w, acc, a.fault);
-        }
-      }
-    } else if (kTwoPass) {  // the next generation; folds nothing (the checksums are of the words read)
-#pragma unroll
-      for (int u = 0; u < U; u++) {
-        const uint32_t i = u * kThreads + threadIdx.x;
-        if (i < nw_tile) {
-          stage[i] = pattern_from_key(gsb_word_key(a.first_word + t * TILE + i), key_write);
-          acc.words += 1u;
-        }
-      }
-    } else {
-#pragma unroll
-      for (int u = 0; u < U; u++) {
-        const uint32_t i = u * kThreads + threadIdx.x;
-        if (i < nw_tile) {
-          uint4 v = make_uint4(0, 0, 0, 0);
-          if (OP != GSB_OP_FILL) v = stage[i];
-          const uint4 nw = process_word<OP>(a, v, a.first_word + t * TILE + i, key_expect, key_write, acc);
-          if (OP != GSB_OP_VERIFY) stage[i] = nw;
-        }
-      }
-    }
+    const unsigned long long w0 = a.first_word + t * TILE;
+    const uint32_t key_expect = reads ? expect_key_of(a, w0) : 0u;
+    if (!kTwoPass)
+      process_stage<op_words(OP), U, kRingThreads>(a, stage, w0, nw_tile, rt, key_expect, key_write, acc);
+    else if (reads)  // compare and fold what was read; its words are counted when they are written
+      process_stage<kRead, U, kRingThreads>(a, stage, w0, nw_tile, rt, key_expect, key_write, acc);
+    else  // the next generation; folds nothing (the checksums are of the words read)
+      process_stage<kWrite | kCount, U, kRingThreads>(a, stage, w0, nw_tile, rt, key_expect, key_write, acc);
     if (writes) fence_proxy_async_smem();  // generic-proxy writes -> visible to the bulk engine
-    __syncthreads();  // every thread is done with this stage (reads, and writes + proxy fence)
+    ring_sync();  // every thread of the ring is done with this stage (reads, and writes + proxy fence)
     if (leader) {
       if (kTwoPass) {
         if (writes) {
@@ -726,117 +750,18 @@ __device__ __forceinline__ void bulk_ring(const gsb_kernel_args &a) {
 
 template <int OP, int U, int S>
 __global__ void __launch_bounds__(kThreads) probe_bulk(const gsb_kernel_args a) {
-  bulk_ring<OP, U, S, StaticSchedule>(a);
+  bulk_ring<OP, U, S, 1, StaticSchedule<1>>(a);
 }
 
 template <int OP, int U, int S>
 __global__ void __launch_bounds__(kThreads) probe_bulk_dyn(const gsb_kernel_args a) {
-  bulk_ring<OP, U, S, ClaimedSchedule<OP == GSB_OP_VERIFY_REFILL ? 2 : 1>>(a);
+  bulk_ring<OP, U, S, 1, ClaimedSchedule<OP == GSB_OP_VERIFY_REFILL ? 2 : 1>>(a);
 }
 
-// ---------------------------------------------------------------- BULKW (per-warp TMA rings)
-//
-// Same data path as BULK, but every warp owns a private ring of S stages of WPL*512 bytes and its own
-// mbarriers; lane 0 issues that warp's bulk loads/stores. Nothing on the data path synchronises the
-// CTA (only __syncwarp), so a warp waiting on HBM never holds the other warps at a barrier. The warps
-// of a CTA take adjacent chunks of one contiguous super-tile, which keeps DRAM pages hot.
+// BULKW: one ring per warp, WPL words per lane
 template <int OP, int WPL, int S, int WARPS>
 __global__ void __launch_bounds__(WARPS * 32) probe_bulk_warp(const gsb_kernel_args a) {
-  constexpr unsigned long long TILE = (unsigned long long)WPL * 32;  // words per warp-tile
-  extern __shared__ __align__(128) unsigned char smem_raw[];
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  uint4 *ring = reinterpret_cast<uint4 *>(smem_raw) + (size_t)warp * S * TILE;  // [S][TILE]
-  __shared__ __align__(8) unsigned long long full_bar[WARPS][S];
-  const unsigned long long n_tiles = (a.n_words + TILE - 1) / TILE;
-  // k-th tile of this warp: warps of one CTA sit side by side inside a WARPS*TILE super-tile
-  auto tile_of = [&](unsigned long long k) -> unsigned long long {
-    return (blockIdx.x + k * gridDim.x) * WARPS + warp;
-  };
-  const unsigned long long first = tile_of(0);
-  const unsigned long long stride = (unsigned long long)gridDim.x * WARPS;
-  const unsigned long long my_n = n_tiles > first ? (n_tiles - first + stride - 1) / stride : 0ull;
-  const uint32_t key_write = gsb_seed_key(a.seed_write);
-  uint4 *__restrict__ win = a.base + a.first_word;
-  const bool leader = lane == 0;
-  Acc acc;
-
-  auto tile_words = [&](unsigned long long k) -> uint32_t {
-    const unsigned long long left = a.n_words - tile_of(k) * TILE;
-    return (uint32_t)(left < TILE ? left : TILE);
-  };
-  auto load = [&](unsigned long long k) {  // leader only
-    const int s = (int)(k % S);
-    const uint32_t bytes = tile_words(k) * 16u;
-    mbar_expect_tx(smem_u32(&full_bar[warp][s]), bytes);
-    bulk_g2s(smem_u32(ring + s * TILE), win + tile_of(k) * TILE, bytes, smem_u32(&full_bar[warp][s]));
-  };
-
-  fault_smem_init();
-  if (leader) {
-#pragma unroll
-    for (int s = 0; s < S; s++) mbar_init(smem_u32(&full_bar[warp][s]), 1u);
-    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-  }
-  __syncthreads();  // the shared histogram is zeroed (the only CTA barrier before finish: the data path uses none)
-
-  constexpr int kPrologue = (OP == GSB_OP_VERIFY) ? S : S - 1;
-  if (OP != GSB_OP_FILL && leader) {
-    for (int k = 0; k < kPrologue; k++)
-      if ((unsigned long long)k < my_n) load(k);
-  }
-
-  for (unsigned long long k = 0; k < my_n; k++) {
-    const unsigned long long t = tile_of(k);
-    const int s = (int)(k % S);
-    const uint32_t nw_tile = tile_words(k);
-    uint4 *stage = ring + s * TILE;
-    if (OP == GSB_OP_FILL) {
-      if (leader) bulk_wait_read<S - 1>();  // the store that last read this stage has drained it
-      __syncwarp();
-    } else {
-      mbar_wait(smem_u32(&full_bar[warp][s]), (uint32_t)((k / S) & 1ull));
-    }
-    const uint32_t key_expect = (OP != GSB_OP_FILL) ? expect_key_of(a, a.first_word + t * TILE) : 0u;
-    if (nw_tile == TILE) {
-      uint4 v[WPL];
-      if (OP != GSB_OP_FILL) {
-#pragma unroll
-        for (int u = 0; u < WPL; u++) v[u] = stage[u * 32 + lane];
-      }
-#pragma unroll
-      for (int u = 0; u < WPL; u++) {
-        const uint4 nw = process_word<OP>(a, v[u], a.first_word + t * TILE + u * 32 + lane, key_expect, key_write, acc);
-        if (OP != GSB_OP_VERIFY) stage[u * 32 + lane] = nw;
-      }
-    } else {
-#pragma unroll
-      for (int u = 0; u < WPL; u++) {
-        const uint32_t i = u * 32 + lane;
-        if (i < nw_tile) {
-          uint4 v = make_uint4(0, 0, 0, 0);
-          if (OP != GSB_OP_FILL) v = stage[i];
-          const uint4 nw = process_word<OP>(a, v, a.first_word + t * TILE + i, key_expect, key_write, acc);
-          if (OP != GSB_OP_VERIFY) stage[i] = nw;
-        }
-      }
-    }
-    if (OP != GSB_OP_VERIFY) fence_proxy_async_smem();
-    __syncwarp();  // the whole warp is done with this stage
-    if (leader) {
-      if (OP == GSB_OP_VERIFY) {
-        if (k + S < my_n) load(k + S);
-      } else {
-        bulk_s2g(win + t * TILE, smem_u32(stage), nw_tile * 16u);
-        bulk_commit();
-        if (OP == GSB_OP_VERIFY_REFILL && k + S - 1 < my_n) {
-          if (k >= 1) bulk_wait_read<1>();
-          load(k + S - 1);
-        }
-      }
-    }
-  }
-  if (leader && OP != GSB_OP_VERIFY) bulk_wait_all<0>();
-  finish(a, acc);
+  bulk_ring<OP, WPL, S, WARPS, StaticSchedule<WARPS>>(a);
 }
 
 // ---------------------------------------------------------------- geometry + dispatch
