@@ -53,6 +53,98 @@
 
 namespace {
 
+// ---------------------------------------------------------------- the periodic health checks (not in the reference)
+
+// What a gsb_*_text function writes: asked for its length, then for the text. Empty when it has nothing to say.
+template <typename Text>
+std::string text_of(Text text) {
+  const int64_t need = text(nullptr, 0);
+  if (need <= 0) return "";
+  std::string s((size_t)need, '\0');
+  const int64_t n = text(&s[0], s.size());
+  s.resize(n > 0 ? (size_t)n : 0);
+  return s;
+}
+
+// One GPU's statistics of one check: zero, and the line of a probe that did not run, when they cannot be read
+// (--fake-inventory, or no such GPU).
+struct Probed {
+  uint64_t probes;
+  std::string counters;  // as dump() prints them
+  std::string line;      // gsb_*_text of the most recent probe
+};
+
+template <typename Stats, typename Result>
+Probed probed(uint32_t idx, const std::string &uuid, int (*get)(uint32_t, Stats *),
+              int64_t (*text)(const Result *, const char *, char *, size_t), uint64_t Stats::*replays,
+              uint64_t Stats::*incomplete) {
+  Stats st;
+  if (get(idx, &st) != GSB_OK) memset(&st, 0, sizeof st);
+  std::ostringstream o;
+  o << " probes " << st.probes << " faults " << st.faults;
+  if (replays) o << " replays " << st.*replays;
+  o << " skipped " << st.skipped;
+  if (incomplete) o << " incomplete " << st.*incomplete;
+  return {st.probes, o.str(), text_of([&](char *buf, size_t cap) { return text(&st.last, uuid.c_str(), buf, cap); })};
+}
+
+struct Check {
+  int Flags::*every;    // --probe-*-every: N > 0 turns the check on
+  uint32_t option;      // the library's cadence option the flag sets
+  uint64_t event;       // the event type of its conditions
+  const char *label;    // in the warning
+  const char *keyword;  // in dump()
+  Probed (*probed)(uint32_t idx, const std::string &uuid);
+  std::vector<std::pair<uint64_t, const char *>> conditions;
+  const char *unknown_condition;
+
+  const char *condition_name(uint64_t c) const {
+    for (const auto &k : conditions)
+      if (k.first == c) return k.second;
+    return unknown_condition;
+  }
+};
+
+// in the order the library runs them, which is the order they are logged and dumped in
+const Check kChecks[] = {
+    {&Flags::probe_link_every, GSB_OPT_LINK_PROBE_EVERY_CYCLES, GSB_EVENT_LINK, "PCIe link health", "link",
+     [](uint32_t i, const std::string &u) {
+       return probed<gsb_link_stats>(i, u, gsb_link_stats_get, gsb_link_text, &gsb_link_stats::replays, nullptr);
+     },
+     {{GSB_LINK_CORRUPT, "corrupted data across the link"},
+      {GSB_LINK_FAILED, "link probe failed"},
+      {GSB_LINK_WIDTH_DEGRADED, "link width degraded"},
+      {GSB_LINK_SPEED_DEGRADED, "link speed degraded"}},
+     "link condition ?"},
+    {&Flags::probe_copy_every, GSB_OPT_COPY_PROBE_EVERY_CYCLES, GSB_EVENT_COPY, "copy-engine health", "copy",
+     [](uint32_t i, const std::string &u) {
+       return probed<gsb_copy_stats>(i, u, gsb_copy_stats_get, gsb_copy_text, nullptr, nullptr);
+     },
+     {{GSB_COPY_CORRUPT, "corrupted data after a DMA copy"}, {GSB_COPY_FAILED, "copy probe failed"}},
+     "copy condition ?"},
+    {&Flags::probe_sm_every, GSB_OPT_SM_PROBE_EVERY_CYCLES, GSB_EVENT_SM, "SM compute health", "sm",
+     [](uint32_t i, const std::string &u) {
+       return probed<gsb_sm_stats>(i, u, gsb_sm_stats_get, gsb_sm_text, nullptr, &gsb_sm_stats::incomplete);
+     },
+     {{GSB_SM_CORRUPT, "wrong result on an SM"}, {GSB_SM_FAILED, "SM probe failed"}},
+     "SM condition ?"},
+    {&Flags::probe_cluster_every, GSB_OPT_CLUSTER_PROBE_EVERY_CYCLES, GSB_EVENT_CLUSTER, "SM-to-SM health", "cluster",
+     [](uint32_t i, const std::string &u) {
+       return probed<gsb_cluster_stats>(i, u, gsb_cluster_stats_get, gsb_cluster_text, nullptr,
+                                        &gsb_cluster_stats::incomplete);
+     },
+     {{GSB_CLUSTER_CORRUPT, "wrong word across the SM-to-SM network"}, {GSB_CLUSTER_FAILED, "SM-to-SM probe failed"}},
+     "SM-to-SM condition ?"},
+    {&Flags::probe_atomic_every, GSB_OPT_ATOMIC_PROBE_EVERY_CYCLES, GSB_EVENT_ATOMIC, "L2 atomic health", "atomic",
+     [](uint32_t i, const std::string &u) {
+       return probed<gsb_atomic_stats>(i, u, gsb_atomic_stats_get, gsb_atomic_text, nullptr,
+                                       &gsb_atomic_stats::incomplete);
+     },
+     {{GSB_ATOMIC_CORRUPT, "wrong result of an L2 atomic"}, {GSB_ATOMIC_FAILED, "L2 atomic probe failed"}},
+     "L2 atomic condition ?"},
+};
+constexpr size_t kNumChecks = sizeof kChecks / sizeof kChecks[0];
+
 // ---------------------------------------------------------------- the plugin (server.go)
 class Plugin {
  public:
@@ -416,13 +508,7 @@ class Plugin {
       gsb_set_option(GSB_OPT_INVENTORY_REFRESH_MS, (uint64_t)f_.inventory_refresh_ms);
       gsb_set_option(GSB_OPT_SWEEP_EVERY_CYCLES, (uint64_t)(f_.probe_sweep_every > 0 ? f_.probe_sweep_every : 0));
       gsb_set_option(GSB_OPT_ECC_HEALTH, f_.health_ecc ? 1 : 0);
-      gsb_set_option(GSB_OPT_LINK_PROBE_EVERY_CYCLES, (uint64_t)(f_.probe_link_every > 0 ? f_.probe_link_every : 0));
-      gsb_set_option(GSB_OPT_COPY_PROBE_EVERY_CYCLES, (uint64_t)(f_.probe_copy_every > 0 ? f_.probe_copy_every : 0));
-      gsb_set_option(GSB_OPT_SM_PROBE_EVERY_CYCLES, (uint64_t)(f_.probe_sm_every > 0 ? f_.probe_sm_every : 0));
-      gsb_set_option(GSB_OPT_CLUSTER_PROBE_EVERY_CYCLES,
-                     (uint64_t)(f_.probe_cluster_every > 0 ? f_.probe_cluster_every : 0));
-      gsb_set_option(GSB_OPT_ATOMIC_PROBE_EVERY_CYCLES,
-                     (uint64_t)(f_.probe_atomic_every > 0 ? f_.probe_atomic_every : 0));
+      for (const Check &c : kChecks) gsb_set_option(c.option, (uint64_t)(f_.*c.every > 0 ? f_.*c.every : 0));
       if (gsb_health_start((uint32_t)f_.probe_period_ms, (uint64_t)f_.probe_window_mib << 20) != GSB_OK) {
         // nvidia.go:114-116: a registration error other than "Not Supported" is log.Fatalf
         logf('F', "Fatal error: %s", last_error().c_str());
@@ -431,11 +517,8 @@ class Plugin {
       }
     }
     std::vector<uint64_t> sweeps_seen(uuids_.size(), 0);
-    std::vector<uint64_t> links_seen(uuids_.size(), 0);
-    std::vector<uint64_t> copies_seen(uuids_.size(), 0);
-    std::vector<uint64_t> sms_seen(uuids_.size(), 0);
-    std::vector<uint64_t> clusters_seen(uuids_.size(), 0);
-    std::vector<uint64_t> atomics_seen(uuids_.size(), 0);
+    std::vector<uint64_t> probes_seen[kNumChecks];
+    for (auto &seen : probes_seen) seen.assign(uuids_.size(), 0);
     while (!stopping_) {
       gsb_event ev;
       const int rc = gsb_health_wait(5000, &ev);  // nvidia.go:126
@@ -450,48 +533,13 @@ class Plugin {
           }
         }
       }
-      if (f_.fake_inventory == 0 && f_.probe_link_every > 0) {  // each GPU's most recent link probe, once
+      for (size_t k = 0; k < kNumChecks; k++) {  // each GPU's most recent probe of every check that is on, once
+        if (f_.fake_inventory != 0 || f_.*kChecks[k].every <= 0) continue;
         for (uint32_t i = 0; i < uuids_.size(); i++) {
-          gsb_link_stats ls;
-          if (gsb_link_stats_get(i, &ls) == GSB_OK && ls.probes > links_seen[i]) {
-            links_seen[i] = ls.probes;
-            INFO("%s", link_line(uuids_[i]).c_str());
-          }
-        }
-      }
-      if (f_.fake_inventory == 0 && f_.probe_copy_every > 0) {  // each GPU's most recent copy probe, once
-        for (uint32_t i = 0; i < uuids_.size(); i++) {
-          gsb_copy_stats cs;
-          if (gsb_copy_stats_get(i, &cs) == GSB_OK && cs.probes > copies_seen[i]) {
-            copies_seen[i] = cs.probes;
-            INFO("%s", copy_line(uuids_[i]).c_str());
-          }
-        }
-      }
-      if (f_.fake_inventory == 0 && f_.probe_sm_every > 0) {  // each GPU's most recent SM probe, once
-        for (uint32_t i = 0; i < uuids_.size(); i++) {
-          gsb_sm_stats ss;
-          if (gsb_sm_stats_get(i, &ss) == GSB_OK && ss.probes > sms_seen[i]) {
-            sms_seen[i] = ss.probes;
-            INFO("%s", sm_line(uuids_[i]).c_str());
-          }
-        }
-      }
-      if (f_.fake_inventory == 0 && f_.probe_cluster_every > 0) {  // each GPU's most recent SM-to-SM probe, once
-        for (uint32_t i = 0; i < uuids_.size(); i++) {
-          gsb_cluster_stats cs;
-          if (gsb_cluster_stats_get(i, &cs) == GSB_OK && cs.probes > clusters_seen[i]) {
-            clusters_seen[i] = cs.probes;
-            INFO("%s", cluster_line(uuids_[i]).c_str());
-          }
-        }
-      }
-      if (f_.fake_inventory == 0 && f_.probe_atomic_every > 0) {  // each GPU's most recent L2 atomic probe, once
-        for (uint32_t i = 0; i < uuids_.size(); i++) {
-          gsb_atomic_stats as;
-          if (gsb_atomic_stats_get(i, &as) == GSB_OK && as.probes > atomics_seen[i]) {
-            atomics_seen[i] = as.probes;
-            INFO("%s", atomic_line(uuids_[i]).c_str());
+          const Probed p = kChecks[k].probed(i, uuids_[i]);
+          if (p.probes > probes_seen[k][i]) {
+            probes_seen[k][i] = p.probes;
+            INFO("%s", p.line.c_str());
           }
         }
       }
@@ -508,33 +556,12 @@ class Plugin {
         mark_unhealthy(ev.uuid);
         continue;
       }
-      if (ev.etype == GSB_EVENT_LINK && f_.probe_link_every > 0) {  // not in the reference: the GPU's host link
-        WARN("PCIe link health of %s: %s: marking it unhealthy", ev.uuid, link_condition_name(ev.edata));
-        WARN("%s", link_line(ev.uuid).c_str());
-        mark_unhealthy(ev.uuid);
-        continue;
-      }
-      if (ev.etype == GSB_EVENT_COPY && f_.probe_copy_every > 0) {  // not in the reference: the GPU's DMA copy engines
-        WARN("copy-engine health of %s: %s: marking it unhealthy", ev.uuid, copy_condition_name(ev.edata));
-        WARN("%s", copy_line(ev.uuid).c_str());
-        mark_unhealthy(ev.uuid);
-        continue;
-      }
-      if (ev.etype == GSB_EVENT_SM && f_.probe_sm_every > 0) {  // not in the reference: what the GPU's SMs compute
-        WARN("SM compute health of %s: %s: marking it unhealthy", ev.uuid, sm_condition_name(ev.edata));
-        WARN("%s", sm_line(ev.uuid).c_str());
-        mark_unhealthy(ev.uuid);
-        continue;
-      }
-      if (ev.etype == GSB_EVENT_CLUSTER && f_.probe_cluster_every > 0) {  // not in the reference: the SM-to-SM network
-        WARN("SM-to-SM health of %s: %s: marking it unhealthy", ev.uuid, cluster_condition_name(ev.edata));
-        WARN("%s", cluster_line(ev.uuid).c_str());
-        mark_unhealthy(ev.uuid);
-        continue;
-      }
-      if (ev.etype == GSB_EVENT_ATOMIC && f_.probe_atomic_every > 0) {  // not in the reference: the L2's atomic units
-        WARN("L2 atomic health of %s: %s: marking it unhealthy", ev.uuid, atomic_condition_name(ev.edata));
-        WARN("%s", atomic_line(ev.uuid).c_str());
+      const Check *check = nullptr;
+      for (const Check &c : kChecks)
+        if (ev.etype == c.event && f_.*c.every > 0) check = &c;
+      if (check) {
+        WARN("%s of %s: %s: marking it unhealthy", check->label, ev.uuid, check->condition_name(ev.edata));
+        WARN("%s", check->probed(gpu_index(ev.uuid), ev.uuid).line.c_str());
         mark_unhealthy(ev.uuid);
         continue;
       }
@@ -830,13 +857,7 @@ class Plugin {
   std::string fault_report_line(uint32_t idx, uint32_t which) {
     gsb_fault_report r;
     if (idx >= uuids_.size() || gsb_fault_report_get(idx, which, &r) != GSB_OK || !r.valid) return "";
-    const int64_t need = gsb_fault_report_text(&r, uuids_[idx].c_str(), nullptr, 0);
-    if (need <= 0) return "";
-    std::string s((size_t)need, '\0');
-    const int64_t n = gsb_fault_report_text(&r, uuids_[idx].c_str(), &s[0], s.size());
-    if (n < 0) return "";
-    s.resize((size_t)n);
-    return s;
+    return text_of([&](char *buf, size_t cap) { return gsb_fault_report_text(&r, uuids_[idx].c_str(), buf, cap); });
   }
   static const char *ecc_condition_name(uint64_t c) {
     switch (c) {
@@ -846,120 +867,18 @@ class Plugin {
       default: return "ECC condition ?";
     }
   }
-  static const char *link_condition_name(uint64_t c) {
-    switch (c) {
-      case GSB_LINK_CORRUPT: return "corrupted data across the link";
-      case GSB_LINK_FAILED: return "link probe failed";
-      case GSB_LINK_WIDTH_DEGRADED: return "link width degraded";
-      case GSB_LINK_SPEED_DEGRADED: return "link speed degraded";
-      default: return "link condition ?";
-    }
-  }
-  static const char *copy_condition_name(uint64_t c) {
-    switch (c) {
-      case GSB_COPY_CORRUPT: return "corrupted data after a DMA copy";
-      case GSB_COPY_FAILED: return "copy probe failed";
-      default: return "copy condition ?";
-    }
-  }
-  // gsb_copy_text of GPU `uuid`'s most recent copy probe; "not run" when there is none (--fake-inventory)
-  std::string copy_line(const std::string &uuid) {
-    gsb_copy_stats st;
-    memset(&st, 0, sizeof st);
-    for (uint32_t i = 0; i < uuids_.size(); i++)
-      if (uuids_[i] == uuid && gsb_copy_stats_get(i, &st) != GSB_OK) memset(&st, 0, sizeof st);
-    const int64_t need = gsb_copy_text(&st.last, uuid.c_str(), nullptr, 0);
-    if (need <= 0) return "";
-    std::string s((size_t)need, '\0');
-    const int64_t n = gsb_copy_text(&st.last, uuid.c_str(), &s[0], s.size());
-    s.resize(n > 0 ? (size_t)n : 0);
-    return s;
-  }
-  static const char *sm_condition_name(uint64_t c) {
-    switch (c) {
-      case GSB_SM_CORRUPT: return "wrong result on an SM";
-      case GSB_SM_FAILED: return "SM probe failed";
-      default: return "SM condition ?";
-    }
-  }
-  // gsb_sm_text of GPU `uuid`'s most recent SM probe; "not run" when there is none (--fake-inventory)
-  std::string sm_line(const std::string &uuid) {
-    gsb_sm_stats st;
-    memset(&st, 0, sizeof st);
-    for (uint32_t i = 0; i < uuids_.size(); i++)
-      if (uuids_[i] == uuid && gsb_sm_stats_get(i, &st) != GSB_OK) memset(&st, 0, sizeof st);
-    const int64_t need = gsb_sm_text(&st.last, uuid.c_str(), nullptr, 0);
-    if (need <= 0) return "";
-    std::string s((size_t)need, '\0');
-    const int64_t n = gsb_sm_text(&st.last, uuid.c_str(), &s[0], s.size());
-    s.resize(n > 0 ? (size_t)n : 0);
-    return s;
-  }
-  static const char *cluster_condition_name(uint64_t c) {
-    switch (c) {
-      case GSB_CLUSTER_CORRUPT: return "wrong word across the SM-to-SM network";
-      case GSB_CLUSTER_FAILED: return "SM-to-SM probe failed";
-      default: return "SM-to-SM condition ?";
-    }
-  }
-  static const char *atomic_condition_name(uint64_t c) {
-    switch (c) {
-      case GSB_ATOMIC_CORRUPT: return "wrong result of an L2 atomic";
-      case GSB_ATOMIC_FAILED: return "L2 atomic probe failed";
-      default: return "L2 atomic condition ?";
-    }
-  }
-  // gsb_atomic_text of GPU `uuid`'s most recent L2 atomic probe; "not run" when there is none (--fake-inventory)
-  std::string atomic_line(const std::string &uuid) {
-    gsb_atomic_stats st;
-    memset(&st, 0, sizeof st);
-    for (uint32_t i = 0; i < uuids_.size(); i++)
-      if (uuids_[i] == uuid && gsb_atomic_stats_get(i, &st) != GSB_OK) memset(&st, 0, sizeof st);
-    const int64_t need = gsb_atomic_text(&st.last, uuid.c_str(), nullptr, 0);
-    if (need <= 0) return "";
-    std::string s((size_t)need, '\0');
-    const int64_t n = gsb_atomic_text(&st.last, uuid.c_str(), &s[0], s.size());
-    s.resize(n > 0 ? (size_t)n : 0);
-    return s;
-  }
-  // gsb_cluster_text of GPU `uuid`'s most recent SM-to-SM probe; "not run" when there is none (--fake-inventory)
-  std::string cluster_line(const std::string &uuid) {
-    gsb_cluster_stats st;
-    memset(&st, 0, sizeof st);
-    for (uint32_t i = 0; i < uuids_.size(); i++)
-      if (uuids_[i] == uuid && gsb_cluster_stats_get(i, &st) != GSB_OK) memset(&st, 0, sizeof st);
-    const int64_t need = gsb_cluster_text(&st.last, uuid.c_str(), nullptr, 0);
-    if (need <= 0) return "";
-    std::string s((size_t)need, '\0');
-    const int64_t n = gsb_cluster_text(&st.last, uuid.c_str(), &s[0], s.size());
-    s.resize(n > 0 ? (size_t)n : 0);
-    return s;
-  }
-  // gsb_link_text of GPU `uuid`'s most recent link probe; every reading "unknown" when there is none (--fake-inventory)
-  std::string link_line(const std::string &uuid) {
-    gsb_link_stats st;
-    memset(&st, 0, sizeof st);
-    for (uint32_t i = 0; i < uuids_.size(); i++)
-      if (uuids_[i] == uuid && gsb_link_stats_get(i, &st) != GSB_OK) memset(&st, 0, sizeof st);
-    const int64_t need = gsb_link_text(&st.last, uuid.c_str(), nullptr, 0);
-    if (need <= 0) return "";
-    std::string s((size_t)need, '\0');
-    const int64_t n = gsb_link_text(&st.last, uuid.c_str(), &s[0], s.size());
-    s.resize(n > 0 ? (size_t)n : 0);
-    return s;
+  // the GPU's place in uuids_; uuids_.size() when it has none
+  uint32_t gpu_index(const std::string &uuid) const {
+    uint32_t i = 0;
+    while (i < uuids_.size() && uuids_[i] != uuid) i++;
+    return i;
   }
   // gsb_ecc_status_text of GPU `uuid`'s live status; every field "unknown" when it cannot be read (--fake-inventory)
   std::string ecc_status_line(const std::string &uuid) {
     gsb_ecc_status st;
     memset(&st, 0, sizeof st);
-    for (uint32_t i = 0; i < uuids_.size(); i++)
-      if (uuids_[i] == uuid && gsb_ecc_status_get(i, &st) != GSB_OK) memset(&st, 0, sizeof st);
-    const int64_t need = gsb_ecc_status_text(&st, uuid.c_str(), nullptr, 0);
-    if (need <= 0) return "";
-    std::string s((size_t)need, '\0');
-    const int64_t n = gsb_ecc_status_text(&st, uuid.c_str(), &s[0], s.size());
-    s.resize(n > 0 ? (size_t)n : 0);
-    return s;
+    if (gsb_ecc_status_get(gpu_index(uuid), &st) != GSB_OK) memset(&st, 0, sizeof st);
+    return text_of([&](char *buf, size_t cap) { return gsb_ecc_status_text(&st, uuid.c_str(), buf, cap); });
   }
   std::string dump() {
     std::lock_guard<std::mutex> lk(hmu_);
@@ -988,49 +907,11 @@ class Plugin {
         o << " " << ecc_status_line(uuids_[g]) << "\n";
       }
     }
-    if (f_.probe_link_every > 0) {  // per GPU: the link probes so far, then the most recent one's line
+    for (const Check &c : kChecks) {  // per GPU and check that is on: the probes so far, then the most recent one's line
+      if (f_.*c.every <= 0) continue;
       for (size_t g = 0; g < uuids_.size(); g++) {
-        gsb_link_stats ls;
-        memset(&ls, 0, sizeof ls);
-        if (gsb_link_stats_get((uint32_t)g, &ls) != GSB_OK) memset(&ls, 0, sizeof ls);
-        o << "link " << uuids_[g] << " probes " << ls.probes << " faults " << ls.faults << " replays " << ls.replays
-          << " skipped " << ls.skipped << "; " << link_line(uuids_[g]) << "\n";
-      }
-    }
-    if (f_.probe_copy_every > 0) {  // per GPU: the copy probes so far, then the most recent one's line
-      for (size_t g = 0; g < uuids_.size(); g++) {
-        gsb_copy_stats cs;
-        memset(&cs, 0, sizeof cs);
-        if (gsb_copy_stats_get((uint32_t)g, &cs) != GSB_OK) memset(&cs, 0, sizeof cs);
-        o << "copy " << uuids_[g] << " probes " << cs.probes << " faults " << cs.faults << " skipped " << cs.skipped
-          << "; " << copy_line(uuids_[g]) << "\n";
-      }
-    }
-    if (f_.probe_sm_every > 0) {  // per GPU: the SM probes so far, then the most recent one's line
-      for (size_t g = 0; g < uuids_.size(); g++) {
-        gsb_sm_stats ss;
-        memset(&ss, 0, sizeof ss);
-        if (gsb_sm_stats_get((uint32_t)g, &ss) != GSB_OK) memset(&ss, 0, sizeof ss);
-        o << "sm " << uuids_[g] << " probes " << ss.probes << " faults " << ss.faults << " skipped " << ss.skipped
-          << " incomplete " << ss.incomplete << "; " << sm_line(uuids_[g]) << "\n";
-      }
-    }
-    if (f_.probe_cluster_every > 0) {  // per GPU: the SM-to-SM probes so far, then the most recent one's line
-      for (size_t g = 0; g < uuids_.size(); g++) {
-        gsb_cluster_stats cs;
-        memset(&cs, 0, sizeof cs);
-        if (gsb_cluster_stats_get((uint32_t)g, &cs) != GSB_OK) memset(&cs, 0, sizeof cs);
-        o << "cluster " << uuids_[g] << " probes " << cs.probes << " faults " << cs.faults << " skipped " << cs.skipped
-          << " incomplete " << cs.incomplete << "; " << cluster_line(uuids_[g]) << "\n";
-      }
-    }
-    if (f_.probe_atomic_every > 0) {  // per GPU: the L2 atomic probes so far, then the most recent one's line
-      for (size_t g = 0; g < uuids_.size(); g++) {
-        gsb_atomic_stats as;
-        memset(&as, 0, sizeof as);
-        if (gsb_atomic_stats_get((uint32_t)g, &as) != GSB_OK) memset(&as, 0, sizeof as);
-        o << "atomic " << uuids_[g] << " probes " << as.probes << " faults " << as.faults << " skipped " << as.skipped
-          << " incomplete " << as.incomplete << "; " << atomic_line(uuids_[g]) << "\n";
+        const Probed p = c.probed((uint32_t)g, uuids_[g]);
+        o << c.keyword << " " << uuids_[g] << p.counters << "; " << p.line << "\n";
       }
     }
     o << "health events queued " << pending_.size() << "\n";

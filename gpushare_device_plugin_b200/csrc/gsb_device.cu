@@ -30,6 +30,7 @@
 #include <time.h>
 
 #include <algorithm>
+#include <array>
 #include <atomic>
 #include <chrono>
 #include <condition_variable>
@@ -41,6 +42,8 @@
 #include <shared_mutex>
 #include <string>
 #include <thread>
+#include <tuple>
+#include <utility>
 #include <vector>
 
 #include "gsb_atomic.h"
@@ -168,6 +171,15 @@ struct Job {
   int rc = 0;
 };
 
+// What a device keeps for one periodic health check (kChecks). stats, raised and hooks are guarded by smu, seed by mu.
+template <typename Stats, typename Hooks>
+struct CheckState {
+  Stats stats{};        // since gsb_health_start (the check's probe calls outside a session count too)
+  uint32_t raised = 0;  // conditions already raised this health session
+  uint32_t seed = 0;    // seeds handed out to the check's probes
+  Hooks hooks{};        // gsb_test_* hooks: applied by the check's next probe, then dropped
+};
+
 struct Device {
   nvmlDevice_t nvml{};
   int ordinal = -1;
@@ -215,30 +227,27 @@ struct Device {
   gsb_ecc_stats ecc_stats{};      // prober thread of this device
   bool ecc_override_set = false;  // gsb_test_ecc_override
   gsb_ecc_status ecc_override{};
-  // PCIe link health; guarded by smu
-  gsb_link_stats link_stats{};     // since gsb_health_start (gsb_link_probe calls outside a session count too)
-  uint32_t link_raised = 0;        // GSB_LINK_* conditions already raised this session
-  bool link_override_set = false;  // gsb_test_link_override
-  gsb_link_status link_override{};
+  // PCIe link health
   struct LinkCorrupt {
     uint32_t phase;
     uint64_t offset;
     uint32_t xr[4];
   };
-  std::vector<LinkCorrupt> link_corrupt;  // gsb_test_link_corrupt: applied by the next gsb_link_probe, then dropped
-  uint32_t link_seed = 0;                 // seeds handed out to link probes (guarded by mu)
+  CheckState<gsb_link_stats, std::vector<LinkCorrupt>> link;  // hooks: gsb_test_link_corrupt
+  bool link_override_set = false;                             // gsb_test_link_override; guarded by smu
+  gsb_link_status link_override{};
   void *link_kept[2] = {nullptr, nullptr};  // pinned buffers a wedged link launch still uses (guarded by mu)
-  // copy-engine health; stats, raised, hooks guarded by smu
-  gsb_copy_stats copy_stats{};  // since gsb_health_start (gsb_copy_probe calls outside a session count too)
-  uint32_t copy_raised = 0;     // GSB_COPY_* conditions already raised this session
+  // copy-engine health
   struct CopyCorrupt {
     uint32_t dir;
     uint64_t offset;
     uint32_t xr[4];
   };
-  std::vector<CopyCorrupt> copy_corrupt;  // gsb_test_copy_corrupt: applied by the next gsb_copy_probe, then dropped
-  uint32_t copy_skip = 0;                 // gsb_test_copy_skip: bit k = direction k's copy is not issued, once
-  uint32_t copy_seed = 0;                 // seeds handed out to copy probes (guarded by mu)
+  struct CopyHooks {
+    std::vector<CopyCorrupt> corrupt;  // gsb_test_copy_corrupt
+    uint32_t skip = 0;                 // gsb_test_copy_skip: bit k = direction k's copy is not issued, once
+  };
+  CheckState<gsb_copy_stats, CopyHooks> copy;
   // the H2D and D2H copies' streams (the D2D copy runs on `stream`) and each copy's timing events, made by the first
   // copy probe (guarded by mu)
   cudaStream_t copy_streams[2] = {nullptr, nullptr};
@@ -246,45 +255,40 @@ struct Device {
   // buffers a wedged copy or verify still uses, given back once every stream has drained (guarded by mu)
   void *copy_kept_dev[3] = {nullptr, nullptr, nullptr};
   void *copy_kept_host[2] = {nullptr, nullptr};
-  // SM compute health; stats, raised, hooks guarded by smu
-  gsb_sm_stats sm_stats{};  // since gsb_health_start (gsb_sm_probe calls outside a session count too)
-  uint32_t sm_raised = 0;   // GSB_SM_* conditions already raised this session
+  // SM compute health (the SM stress takes its seeds from the same counter)
   struct SmCorrupt {
     bool armed = false;
     uint32_t smid = 0, index = 0;
     uint64_t xr = 0;
   };
-  SmCorrupt sm_corrupt[GSB_SM_UNITS];  // gsb_test_sm_corrupt: applied by the next gsb_sm_probe, then dropped
-  // gsb_test_sm_operands: per tensor unit, the 8192 expected D words then the operand table (gsb_sm_table_*), taken by
-  // the next gsb_sm_probe that runs the unit; empty = not armed
-  std::vector<uint32_t> sm_operands[GSB_SM_UNITS];
-  uint32_t sm_seed = 0;                // seeds handed out to SM probes (guarded by mu)
-  void *sm_kept = nullptr;             // buffer a wedged SM-check or SM-stress launch still uses (guarded by mu)
+  struct SmHooks {
+    std::array<SmCorrupt, GSB_SM_UNITS> corrupt;  // gsb_test_sm_corrupt
+    // gsb_test_sm_operands: per tensor unit, the 8192 expected D words then the operand table (gsb_sm_table_*), taken
+    // by the next gsb_sm_probe that runs the unit; empty = not armed
+    std::vector<uint32_t> operands[GSB_SM_UNITS];
+  };
+  CheckState<gsb_sm_stats, SmHooks> sm;
+  // buffer a wedged SM-check, SM-stress, SM-to-SM or L2 atomic launch still uses (guarded by mu)
+  void *sm_kept = nullptr;
   struct StressCorrupt {
     bool armed = false;
     uint32_t smid = 0, unit = 0, index = 0, xr = 0, slice = 0;
   };
   StressCorrupt stress_corrupt;  // gsb_test_stress_corrupt: applied by the next gsb_sm_stress, then dropped (smu)
-  // SM-to-SM health; stats, raised, hooks guarded by smu (a wedged launch's buffer is kept in sm_kept)
-  gsb_cluster_stats cluster_stats{};  // since gsb_health_start (gsb_cluster_probe calls outside a session count too)
-  uint32_t cluster_raised = 0;        // GSB_CLUSTER_* conditions already raised this session
+  // SM-to-SM health
   struct ClusterHook {
     bool corrupt = false, skip = false;
     uint32_t corrupt_smid = 0, index = 0, skip_smid = 0;
     uint64_t xr = 0;
   };
-  ClusterHook cluster_hook[GSB_CLUSTER_PATHS];  // gsb_test_cluster_*: applied by the next gsb_cluster_probe, then dropped
-  uint32_t cluster_seed = 0;                    // seeds handed out to cluster probes (guarded by mu)
-  // L2 atomic health; stats, raised, hooks guarded by smu (a wedged launch's buffer is kept in sm_kept)
-  gsb_atomic_stats atomic_stats{};  // since gsb_health_start (gsb_atomic_probe calls outside a session count too)
-  uint32_t atomic_raised = 0;       // GSB_ATOMIC_* conditions already raised this session
+  CheckState<gsb_cluster_stats, std::array<ClusterHook, GSB_CLUSTER_PATHS>> cluster;  // hooks: gsb_test_cluster_*
+  // L2 atomic health
   struct AtomicHook {
     bool corrupt = false, skip = false;
     uint32_t word = 0, skip_smid = 0;
     uint64_t xr = 0;
   };
-  AtomicHook atomic_hook[GSB_ATOMIC_OPS];  // gsb_test_atomic_*: applied by the next gsb_atomic_probe, then dropped
-  uint32_t atomic_seed = 0;                // seeds handed out to atomic probes (guarded by mu)
+  CheckState<gsb_atomic_stats, std::array<AtomicHook, GSB_ATOMIC_OPS>> atomic;  // hooks: gsb_test_atomic_*
 
   // persistent worker (gsb_cycle_all / gsb_probe_all): one host thread per device
   std::thread worker;
@@ -314,11 +318,7 @@ struct Global {
   std::atomic<uint64_t> transient_keep_free{1ull << 30};
   std::atomic<uint64_t> sweep_every{0};
   std::atomic<uint64_t> ecc_health{0};
-  std::atomic<uint64_t> link_every{0};
-  std::atomic<uint64_t> copy_every{0};
-  std::atomic<uint64_t> sm_every{0};
-  std::atomic<uint64_t> cluster_every{0};
-  std::atomic<uint64_t> atomic_every{0};
+  std::atomic<uint64_t> check_every[5] = {};  // GSB_OPT_*_PROBE_EVERY_CYCLES, by the check's place in Checks
 
   // one link or copy probe's pinned buffers at a time in the whole process (the DaemonSet's memory limit covers 8 GPUs)
   std::mutex link_mu;
@@ -1101,6 +1101,65 @@ void push_event(const gsb_event &ev) {
   G.hcv.notify_all();
 }
 
+// ------------------------------------------------------------------ what every health check does the same way
+
+// Raise every condition of `conditions()` (evaluated under smu) that this device has not raised yet: one event of
+// `etype` per condition per device per health session.
+template <typename Conditions>
+void raise_conditions(Device *d, uint64_t etype, uint32_t *raised, Conditions conditions) {
+  uint32_t fresh;
+  {
+    std::lock_guard<std::mutex> lk(d->smu);
+    fresh = conditions() & ~*raised;
+    *raised |= fresh;
+  }
+  for (uint32_t bit = 1; fresh; bit <<= 1) {
+    if (!(fresh & bit)) continue;
+    fresh &= ~bit;
+    gsb_event ev;
+    memset(&ev, 0, sizeof ev);
+    snprintf(ev.uuid, sizeof ev.uuid, "%s", d->uuid);
+    ev.etype = etype;
+    ev.edata = bit;
+    push_event(ev);
+  }
+}
+
+// The statistics of one finished probe. A probe that ran nothing learnt nothing and counts as skipped; `incomplete`
+// is the check's counter of probes that covered less than they should have, or null when this one covered it all (the
+// link and copy checks have no such counter).
+template <typename Stats, typename Result>
+void count_probe(Device *d, Stats *st, const Result &r, bool ran, uint32_t conditions, uint64_t *incomplete = nullptr) {
+  std::lock_guard<std::mutex> lk(d->smu);
+  st->probes++;
+  if (!ran) st->skipped++;
+  if (incomplete) ++*incomplete;
+  if (conditions) st->faults++;
+  st->last = r;
+}
+
+// The armed test hooks, disarmed: a hook applies to the next probe only.
+template <typename Hooks>
+Hooks take_hooks(Device *d, Hooks *armed) {
+  std::lock_guard<std::mutex> lk(d->smu);
+  return std::exchange(*armed, Hooks{});
+}
+
+// The seed the caller gave or, for 0, a fresh one: old data then reads as stale, and no two probes share operands.
+uint32_t seed_or_fresh(uint32_t given, uint32_t base, uint32_t *handed_out, uint32_t stride = 1) {
+  return given ? given : base + stride * ++*handed_out;
+}
+
+// A launch that outlived the watchdog is still on the device's stream: nothing is queued behind it until it drained.
+int wedged_drain_locked(Device *d) {
+  if (cudaStreamQuery(d->stream) == cudaErrorNotReady) {
+    set_error("%s: an earlier launch is still running (wedged)", d->uuid);
+    return GSB_ERR_TIMEOUT;
+  }
+  d->wedged = false;
+  return GSB_OK;
+}
+
 // ------------------------------------------------------------------ ECC health
 
 uint64_t realtime_ns() {
@@ -1194,22 +1253,7 @@ bool read_ecc_totals(Device *d, uint64_t *corrected, uint64_t *uncorrected) {
 // Raise every condition of `now` against the session's baseline that this device has not raised yet (one event per
 // condition per device per health session).
 void raise_ecc_conditions(Device *d, const gsb_ecc_status &now) {
-  uint32_t fresh;
-  {
-    std::lock_guard<std::mutex> lk(d->smu);
-    fresh = gsb_ecc_conditions(&d->ecc_baseline, &now) & ~d->ecc_raised;
-    d->ecc_raised |= fresh;
-  }
-  for (uint32_t bit = 1; fresh; bit <<= 1) {
-    if (!(fresh & bit)) continue;
-    fresh &= ~bit;
-    gsb_event ev;
-    memset(&ev, 0, sizeof ev);
-    snprintf(ev.uuid, sizeof ev.uuid, "%s", d->uuid);
-    ev.etype = GSB_EVENT_ECC;
-    ev.edata = bit;
-    push_event(ev);
-  }
+  raise_conditions(d, GSB_EVENT_ECC, &d->ecc_raised, [&] { return gsb_ecc_conditions(&d->ecc_baseline, &now); });
 }
 
 struct EccPrev {  // a prober thread's last valid post-cycle read
@@ -1408,7 +1452,7 @@ void query_link(Device *d, gsb_link_status *out, uint32_t what = ~0u) {
   bool overridden;
   {
     std::lock_guard<std::mutex> lk(d->smu);
-    d->link_stats.queries++;
+    d->link.stats.queries++;
     overridden = d->link_override_set;
     if (overridden) {
       *out = d->link_override;
@@ -1465,28 +1509,18 @@ int link_probe_locked(Device *d, const gsb_link_cfg *cfg, gsb_link_result *out) 
     return out->status = GSB_ERR_INVALID_ARGUMENT;
   }
   int rc = ensure_ready(d);
+  if (!rc && d->wedged) rc = wedged_drain_locked(d);
   if (rc) return out->status = rc;
-  if (d->wedged) {  // a launch that outlived the watchdog: queue nothing behind it until it has drained
-    if (cudaStreamQuery(d->stream) == cudaErrorNotReady) {
-      set_error("%s: an earlier launch is still running (wedged)", d->uuid);
-      return out->status = GSB_ERR_TIMEOUT;
-    }
-    d->wedged = false;
-  }
   for (void *&p : d->link_kept) {  // buffers a wedged link launch kept: the stream has drained, give them back
     if (p) cudaFreeHost(p);
     p = nullptr;
   }
   out->passes = passes;
   out->buffer_bytes = L;
-  if (!cfg->seed_a || !cfg->seed_b) d->link_seed += 2;
-  out->seed_a = cfg->seed_a ? cfg->seed_a : 0x4C4E0000u + d->link_seed;  // fresh per probe: old data reads as STALE
-  out->seed_b = cfg->seed_b ? cfg->seed_b : 0x4C4E0001u + d->link_seed;
-  std::vector<Device::LinkCorrupt> corrupt;
-  {
-    std::lock_guard<std::mutex> lk(d->smu);
-    corrupt.swap(d->link_corrupt);
-  }
+  if (!cfg->seed_a || !cfg->seed_b) d->link.seed += 2;
+  out->seed_a = cfg->seed_a ? cfg->seed_a : 0x4C4E0000u + d->link.seed;  // fresh per probe: old data reads as STALE
+  out->seed_b = cfg->seed_b ? cfg->seed_b : 0x4C4E0001u + d->link.seed;
+  const std::vector<Device::LinkCorrupt> corrupt = take_hooks(d, &d->link.hooks);
   query_link(d, &out->idle);  // at idle, before any probe traffic: current, maximum, replay counter
 
   std::lock_guard<std::mutex> one(G.link_mu);
@@ -1609,36 +1643,12 @@ int link_probe_locked(Device *d, const gsb_link_cfg *cfg, gsb_link_result *out) 
   out->link_gbps = (out->load_valid & both) == both ? gsb_link_rate_gbps(out->load_gen, out->load_width) : 0.0;
   out->wall_ns = now_ns() - t0;
   out->status = rc;
-  {
+  if (out->replay_valid) {
     std::lock_guard<std::mutex> lk(d->smu);
-    gsb_link_stats &ls = d->link_stats;
-    ls.probes++;
-    if (out->phases[0].op == 0) ls.skipped++;  // no phase ran: nothing was learnt about the link
-    if (gsb_link_conditions(out)) ls.faults++;
-    if (out->replay_valid) ls.replays += out->replays;
-    ls.last = *out;
+    d->link.stats.replays += out->replays;
   }
+  count_probe(d, &d->link.stats, *out, out->phases[0].op != 0, gsb_link_conditions(out));
   return rc;
-}
-
-// Raise every condition of `r` this device has not raised yet this health session (one event per condition).
-void raise_link_conditions(Device *d, const gsb_link_result &r) {
-  uint32_t fresh;
-  {
-    std::lock_guard<std::mutex> lk(d->smu);
-    fresh = gsb_link_conditions(&r) & ~d->link_raised;
-    d->link_raised |= fresh;
-  }
-  for (uint32_t bit = 1; fresh; bit <<= 1) {
-    if (!(fresh & bit)) continue;
-    fresh &= ~bit;
-    gsb_event ev;
-    memset(&ev, 0, sizeof ev);
-    snprintf(ev.uuid, sizeof ev.uuid, "%s", d->uuid);
-    ev.etype = GSB_EVENT_LINK;
-    ev.edata = bit;
-    push_event(ev);
-  }
 }
 
 // ------------------------------------------------------------------ copy-engine health (gsb_copy_probe)
@@ -1763,18 +1773,13 @@ int copy_probe_locked(Device *d, const gsb_copy_cfg *cfg, gsb_copy_result *out) 
   int engines = 0;
   if (cudaDeviceGetAttribute(&engines, cudaDevAttrAsyncEngineCount, d->ordinal) == cudaSuccess)
     out->async_engines = (uint32_t)engines;
-  if (!cfg->seed_src || !cfg->seed_host || !cfg->seed_bg) d->copy_seed += 3;
-  out->seed_src = cfg->seed_src ? cfg->seed_src : 0x43500000u + d->copy_seed;  // fresh per probe: old data reads STALE
-  out->seed_host = cfg->seed_host ? cfg->seed_host : 0x43500001u + d->copy_seed;
-  out->seed_bg = cfg->seed_bg ? cfg->seed_bg : 0x43500002u + d->copy_seed;
-  std::vector<Device::CopyCorrupt> corrupt;
-  uint32_t skip;
-  {
-    std::lock_guard<std::mutex> lk(d->smu);
-    corrupt.swap(d->copy_corrupt);
-    skip = d->copy_skip;
-    d->copy_skip = 0;
-  }
+  if (!cfg->seed_src || !cfg->seed_host || !cfg->seed_bg) d->copy.seed += 3;
+  out->seed_src = cfg->seed_src ? cfg->seed_src : 0x43500000u + d->copy.seed;  // fresh per probe: old data reads STALE
+  out->seed_host = cfg->seed_host ? cfg->seed_host : 0x43500001u + d->copy.seed;
+  out->seed_bg = cfg->seed_bg ? cfg->seed_bg : 0x43500002u + d->copy.seed;
+  const Device::CopyHooks hooks = take_hooks(d, &d->copy.hooks);
+  const std::vector<Device::CopyCorrupt> &corrupt = hooks.corrupt;
+  const uint32_t skip = hooks.skip;
 
   std::lock_guard<std::mutex> one(G.link_mu);
   void *dev[3] = {nullptr, nullptr, nullptr};  // S, D_h2d, D_d2d
@@ -1968,35 +1973,8 @@ int copy_probe_locked(Device *d, const gsb_copy_cfg *cfg, gsb_copy_result *out) 
   }
   out->wall_ns = now_ns() - t0;
   out->status = rc;
-  {
-    std::lock_guard<std::mutex> lk(d->smu);
-    gsb_copy_stats &cs = d->copy_stats;
-    cs.probes++;
-    if (out->dirs[0].op == 0) cs.skipped++;  // no direction ran: nothing was learnt about the copy engines
-    if (gsb_copy_conditions(out)) cs.faults++;
-    cs.last = *out;
-  }
+  count_probe(d, &d->copy.stats, *out, out->dirs[0].op != 0, gsb_copy_conditions(out));
   return rc;
-}
-
-// Raise every condition of `r` this device has not raised yet this health session (one event per condition).
-void raise_copy_conditions(Device *d, const gsb_copy_result &r) {
-  uint32_t fresh;
-  {
-    std::lock_guard<std::mutex> lk(d->smu);
-    fresh = gsb_copy_conditions(&r) & ~d->copy_raised;
-    d->copy_raised |= fresh;
-  }
-  for (uint32_t bit = 1; fresh; bit <<= 1) {
-    if (!(fresh & bit)) continue;
-    fresh &= ~bit;
-    gsb_event ev;
-    memset(&ev, 0, sizeof ev);
-    snprintf(ev.uuid, sizeof ev.uuid, "%s", d->uuid);
-    ev.etype = GSB_EVENT_COPY;
-    ev.edata = bit;
-    push_event(ev);
-  }
 }
 
 // ------------------------------------------------------------------ SM compute health (gsb_sm_probe)
@@ -2078,15 +2056,11 @@ int sm_launch_locked(Device *d, uint32_t unit, const gsb_sm_args &args, gsb_sm_l
 
 // Before a new SM check or stress: a launch that outlived the watchdog must have drained (its buffer is given back).
 int sm_drain_kept_locked(Device *d) {
-  if (d->wedged || d->sm_kept) {  // an earlier launch outlived the watchdog: queue nothing behind it until it drained
-    if (cudaStreamQuery(d->stream) == cudaErrorNotReady) {
-      set_error("%s: an earlier launch is still running (wedged)", d->uuid);
-      return GSB_ERR_TIMEOUT;
-    }
-    d->wedged = false;
-    if (d->sm_kept) cudaFree(d->sm_kept);
-    d->sm_kept = nullptr;
-  }
+  if (!d->wedged && !d->sm_kept) return GSB_OK;
+  const int rc = wedged_drain_locked(d);
+  if (rc) return rc;
+  if (d->sm_kept) cudaFree(d->sm_kept);
+  d->sm_kept = nullptr;
   return GSB_OK;
 }
 
@@ -2109,6 +2083,48 @@ int sm_alloc_locked(Device *d, const char *what, size_t bytes, void **buf) {
   return GSB_OK;
 }
 
+// Owns the transient buffer of one SM-side run whose status is `rc`. On release (at the latest when the run returns)
+// the buffer is freed, unless the run ended in GSB_ERR_TIMEOUT: then a launch still on the stream uses it, and it goes
+// to sm_kept, which sm_drain_kept_locked frees once the stream has drained.
+struct SmBuffer {
+  Device *d;
+  const int &rc;
+  void *p = nullptr;
+  SmBuffer(Device *d, const int &rc) : d(d), rc(rc) {}
+  SmBuffer(const SmBuffer &) = delete;
+  ~SmBuffer() { release(); }
+  int alloc(const char *what, size_t bytes) { return sm_alloc_locked(d, what, bytes, &p); }
+  void release() {
+    if (!p) return;
+    if (rc == GSB_ERR_TIMEOUT) d->sm_kept = p;
+    else cudaFree(p);
+    p = nullptr;
+  }
+};
+
+// The most dynamic shared memory a CTA of this device can opt in to.
+int smem_optin_locked(Device *d, int *smem) {
+  if (cudaDeviceGetAttribute(smem, cudaDevAttrMaxSharedMemoryPerBlockOptin, d->ordinal) == cudaSuccess) return GSB_OK;
+  set_error("querying the shared-memory opt-in maximum of %s", d->uuid);
+  return GSB_ERR_DRIVER;
+}
+
+// Folds one launch's log into its run (or unit) and into the probe's result: the words compared and found wrong, the
+// SMs the launch ran on into `covered`, the SMs with a wrong word, and its records while the result has room.
+template <typename Log, typename Run, typename Result>
+void fold_log(const Log &log, Run *run, Result *out, uint32_t *covered) {
+  run->words_checked += log.words;
+  run->mismatch_words += log.mismatch_words;
+  run->mismatch_bits += log.mismatch_bits;
+  for (size_t i = 0; i < std::size(log.covered); i++) {
+    covered[i] |= log.covered[i];
+    out->faulty[i] |= log.faulty[i];
+  }
+  const uint32_t got = std::min<uint32_t>(log.count, std::size(log.rec));
+  for (uint32_t i = 0; i < got && out->n_records < std::size(out->records); i++)
+    out->records[out->n_records++] = log.rec[i];
+}
+
 int sm_probe_locked(Device *d, const gsb_sm_cfg *cfg, gsb_sm_result *out) {
   const uint64_t t0 = now_ns();
   if (cfg->units & ~kSmAllUnits) {
@@ -2120,18 +2136,14 @@ int sm_probe_locked(Device *d, const gsb_sm_cfg *cfg, gsb_sm_result *out) {
   int rc = ensure_ready(d);
   if (!rc) rc = sm_drain_kept_locked(d);
   if (rc) return out->status = rc;
-  if (!cfg->seed) d->sm_seed++;
-  out->seed = cfg->seed ? cfg->seed : 0x534D0000u + d->sm_seed;  // fresh per probe
+  out->seed = seed_or_fresh(cfg->seed, 0x534D0000u, &d->sm.seed);
   out->seed_expect = cfg->seed_expect ? cfg->seed_expect : out->seed;
-  Device::SmCorrupt hooks[GSB_SM_UNITS];
+  const auto hooks = take_hooks(d, &d->sm.hooks.corrupt);
   std::vector<uint32_t> chosen[GSB_SM_UNITS];  // gsb_test_sm_operands of the units this probe runs
   {
     std::lock_guard<std::mutex> lk(d->smu);
-    for (uint32_t u = 0; u < GSB_SM_UNITS; u++) {
-      hooks[u] = d->sm_corrupt[u];
-      d->sm_corrupt[u] = Device::SmCorrupt{};
-      if (out->units >> u & 1u) chosen[u].swap(d->sm_operands[u]);
-    }
+    for (uint32_t u = 0; u < GSB_SM_UNITS; u++)
+      if (out->units >> u & 1u) chosen[u].swap(d->sm.hooks.operands[u]);
   }
   static const SmLayout layout;
   // chosen operands and their expected words go after the tables, one 256-byte aligned block per unit
@@ -2160,33 +2172,31 @@ int sm_probe_locked(Device *d, const gsb_sm_cfg *cfg, gsb_sm_result *out) {
   }
   out->expected_ns = now_ns() - t_exp;
   // one transient buffer: the launch log and the tables, under the keep-free margin of every transient probe
-  void *buf = nullptr;
-  rc = sm_alloc_locked(d, "SM probe", bytes, &buf);
+  SmBuffer buf(d, rc);
+  rc = buf.alloc("SM probe", bytes);
+  char *const base = static_cast<char *>(buf.p);
   if (rc == GSB_OK) {
-    cudaError_t e = cudaMemcpyAsync(static_cast<char *>(buf) + layout.offset[0], &tables[layout.offset[0]],
+    cudaError_t e = cudaMemcpyAsync(base + layout.offset[0], &tables[layout.offset[0]],
                                     layout.bytes - layout.offset[0], cudaMemcpyHostToDevice, d->stream);
     for (uint32_t u = 0; u < GSB_SM_UNITS && e == cudaSuccess; u++)
       if (!chosen[u].empty())
-        e = cudaMemcpyAsync(static_cast<char *>(buf) + chosen_off[u], chosen[u].data(),
-                            chosen[u].size() * sizeof(uint32_t), cudaMemcpyHostToDevice, d->stream);
+        e = cudaMemcpyAsync(base + chosen_off[u], chosen[u].data(), chosen[u].size() * sizeof(uint32_t),
+                            cudaMemcpyHostToDevice, d->stream);
     if (e != cudaSuccess || cudaStreamSynchronize(d->stream) != cudaSuccess) {
       set_error("uploading the SM probe's expected answers to %s: %s", d->uuid, cudaGetErrorString(e));
       rc = GSB_ERR_DRIVER;
     }
   }
   int smem = 0;
-  if (rc == GSB_OK && cudaDeviceGetAttribute(&smem, cudaDevAttrMaxSharedMemoryPerBlockOptin, d->ordinal) != cudaSuccess) {
-    set_error("querying the shared-memory opt-in maximum of %s", d->uuid);
-    rc = GSB_ERR_DRIVER;
-  }
-  bool wedged = false, first = true;
+  if (rc == GSB_OK) rc = smem_optin_locked(d, &smem);
+  bool first = true;
   for (uint32_t u = 0; u < GSB_SM_UNITS && rc == GSB_OK; u++) {
     if (!(out->units >> u & 1u)) continue;
     gsb_sm_unit_result &ur = out->unit[u];
     gsb_sm_args a;
     memset(&a, 0, sizeof a);
-    a.log = static_cast<gsb_sm_log *>(buf);
-    a.expected = static_cast<char *>(buf) + (chosen[u].empty() ? layout.offset[u] : chosen_off[u]);
+    a.log = reinterpret_cast<gsb_sm_log *>(base);
+    a.expected = base + (chosen[u].empty() ? layout.offset[u] : chosen_off[u]);
     a.seed = out->seed;
     a.smem_bytes = (uint32_t)smem;
     a.hook_smid = GSB_SM_MAX;
@@ -2204,65 +2214,26 @@ int sm_probe_locked(Device *d, const gsb_sm_cfg *cfg, gsb_sm_result *out) {
       gsb_sm_log log;
       const int lrc = sm_launch_locked(d, u, a, &log, &ur.kernel_ns, !chosen[u].empty());
       if (lrc != GSB_OK) {
-        ur.status = lrc;
-        rc = lrc;
-        wedged = lrc == GSB_ERR_TIMEOUT;
+        ur.status = rc = lrc;
         break;
       }
-      ur.words_checked += log.words;
-      ur.mismatch_words += log.mismatch_words;
-      ur.mismatch_bits += log.mismatch_bits;
-      for (int i = 0; i < GSB_SM_MAX / 32; i++) {
-        covered[i] |= log.covered[i];
-        out->faulty[i] |= log.faulty[i];
-      }
-      const uint32_t got = log.count < GSB_SM_RECORDS ? log.count : GSB_SM_RECORDS;
-      for (uint32_t i = 0; i < got && out->n_records < GSB_SM_RECORDS; i++) out->records[out->n_records++] = log.rec[i];
+      fold_log(log, &ur, out, covered);
     }
     ur.sms_covered = popcount_bitmap(covered);
     for (int i = 0; i < GSB_SM_MAX / 32; i++) out->covered[i] = first ? covered[i] : out->covered[i] & covered[i];
     first = false;
   }
   out->sms_covered = popcount_bitmap(out->covered);
-  if (wedged) d->sm_kept = buf;  // given back once the stream has drained
-  else if (buf) cudaFree(buf);
+  buf.release();
   out->wall_ns = now_ns() - t0;
   out->status = rc;
-  {
-    std::lock_guard<std::mutex> lk(d->smu);
-    gsb_sm_stats &st = d->sm_stats;
-    st.probes++;
-    bool ran = false, short_cover = false;
-    for (const gsb_sm_unit_result &ur : out->unit) {
-      ran = ran || ur.launches != 0;
-      short_cover = short_cover || (ur.launches != 0 && ur.status == GSB_OK && ur.sms_covered < out->sm_count);
-    }
-    if (!ran) st.skipped++;  // no unit ran: nothing was learnt about the SMs
-    if (short_cover) st.incomplete++;
-    if (gsb_sm_conditions(out)) st.faults++;
-    st.last = *out;
+  bool ran = false, short_cover = false;
+  for (const gsb_sm_unit_result &ur : out->unit) {
+    ran = ran || ur.launches != 0;
+    short_cover = short_cover || (ur.launches != 0 && ur.status == GSB_OK && ur.sms_covered < out->sm_count);
   }
+  count_probe(d, &d->sm.stats, *out, ran, gsb_sm_conditions(out), short_cover ? &d->sm.stats.incomplete : nullptr);
   return rc;
-}
-
-// Raise every condition of `r` this device has not raised yet this health session (one event per condition).
-void raise_sm_conditions(Device *d, const gsb_sm_result &r) {
-  uint32_t fresh;
-  {
-    std::lock_guard<std::mutex> lk(d->smu);
-    fresh = gsb_sm_conditions(&r) & ~d->sm_raised;
-    d->sm_raised |= fresh;
-  }
-  for (uint32_t bit = 1; fresh; bit <<= 1) {
-    if (!(fresh & bit)) continue;
-    fresh &= ~bit;
-    gsb_event ev;
-    memset(&ev, 0, sizeof ev);
-    snprintf(ev.uuid, sizeof ev.uuid, "%s", d->uuid);
-    ev.etype = GSB_EVENT_SM;
-    ev.edata = bit;
-    push_event(ev);
-  }
 }
 
 
@@ -2345,16 +2316,10 @@ int stress_locked(Device *d, const gsb_stress_cfg *cfg, gsb_stress_result *out) 
   int rc = ensure_ready(d);
   if (!rc) rc = sm_drain_kept_locked(d);
   if (rc) return out->status = rc;
-  if (!cfg->seed) d->sm_seed++;
-  // fresh per run, and no two runs share an operand set (set s uses seed + s)
-  out->seed = cfg->seed ? cfg->seed : 0x53540000u + GSB_STRESS_SETS_MAX * d->sm_seed;
+  // no two runs share an operand set (set s uses seed + s)
+  out->seed = seed_or_fresh(cfg->seed, 0x53540000u, &d->sm.seed, GSB_STRESS_SETS_MAX);
   out->seed_expect = cfg->seed_expect ? cfg->seed_expect : out->seed;
-  Device::StressCorrupt hook;
-  {
-    std::lock_guard<std::mutex> lk(d->smu);
-    hook = d->stress_corrupt;
-    d->stress_corrupt = Device::StressCorrupt{};
-  }
+  const Device::StressCorrupt hook = take_hooks(d, &d->stress_corrupt);
   // the buffer: the slice log, every unit's expected folds, then SmLayout's answers, one table per operand set
   const size_t folds_at = (sizeof(gsb_stress_log) + 255) / 256 * 256;
   const size_t fold_set_bytes = GSB_STRESS_FOLD_THREADS * sizeof(uint32_t);
@@ -2376,21 +2341,19 @@ int stress_locked(Device *d, const gsb_stress_cfg *cfg, gsb_stress_result *out) 
     }
   }
   out->expected_ns = now_ns() - t_exp;
-  void *buf = nullptr;
-  rc = sm_alloc_locked(d, "SM stress", layout.bytes, &buf);
+  SmBuffer buf(d, rc);
+  rc = buf.alloc("SM stress", layout.bytes);
+  char *const base = static_cast<char *>(buf.p);
   if (rc == GSB_OK) {
-    const cudaError_t e = cudaMemcpyAsync(static_cast<char *>(buf) + folds_at, &tables[folds_at],
-                                          layout.bytes - folds_at, cudaMemcpyHostToDevice, d->stream);
+    const cudaError_t e = cudaMemcpyAsync(base + folds_at, &tables[folds_at], layout.bytes - folds_at,
+                                          cudaMemcpyHostToDevice, d->stream);
     if (e != cudaSuccess || cudaStreamSynchronize(d->stream) != cudaSuccess) {
       set_error("uploading the SM stress's expected answers to %s: %s", d->uuid, cudaGetErrorString(e));
       rc = GSB_ERR_DRIVER;
     }
   }
   int smem = 0;
-  if (rc == GSB_OK && cudaDeviceGetAttribute(&smem, cudaDevAttrMaxSharedMemoryPerBlockOptin, d->ordinal) != cudaSuccess) {
-    set_error("querying the shared-memory opt-in maximum of %s", d->uuid);
-    rc = GSB_ERR_DRIVER;
-  }
+  if (rc == GSB_OK) rc = smem_optin_locked(d, &smem);
   uint32_t sel[GSB_STRESS_UNITS], nsel = 0;
   for (uint32_t u = GSB_SM_UNIT_F16; u <= GSB_SM_UNIT_S8; u++)
     if (out->units >> u & 1u) sel[nsel++] = u;
@@ -2398,7 +2361,6 @@ int stress_locked(Device *d, const gsb_stress_cfg *cfg, gsb_stress_result *out) 
   if (rc == GSB_OK) sampler.begin();
   const std::function<void()> poll = [&] { sampler.poll(); };
   uint64_t sm_iters[GSB_SM_MAX] = {};
-  bool wedged = false;
   const uint32_t n_slices = (out->duration_ms + out->slice_ms - 1) / out->slice_ms;
   for (uint32_t i = 0; i < n_slices && rc == GSB_OK; i++) {
     const uint32_t u = sel[i % nsel], k = u - GSB_SM_UNIT_F16;
@@ -2406,10 +2368,9 @@ int stress_locked(Device *d, const gsb_stress_cfg *cfg, gsb_stress_result *out) 
     gsb_stress_unit_result &ur = out->unit[k];
     gsb_stress_args a;
     memset(&a, 0, sizeof a);
-    a.log = static_cast<gsb_stress_log *>(buf);
-    a.expected = reinterpret_cast<const uint32_t *>(static_cast<char *>(buf) + layout.offset[u]);
-    a.folds = reinterpret_cast<const uint32_t *>(static_cast<char *>(buf) + folds_at +
-                                                 k * GSB_STRESS_SETS_MAX * fold_set_bytes);
+    a.log = reinterpret_cast<gsb_stress_log *>(base);
+    a.expected = reinterpret_cast<const uint32_t *>(base + layout.offset[u]);
+    a.folds = reinterpret_cast<const uint32_t *>(base + folds_at + k * GSB_STRESS_SETS_MAX * fold_set_bytes);
     a.slice_ns = len_ms * 1000000ull;
     a.max_iters = (uint64_t)len_ms * 1000 * gsb_stress_iters_per_us(u);
     a.seed = out->seed;
@@ -2431,29 +2392,21 @@ int stress_locked(Device *d, const gsb_stress_cfg *cfg, gsb_stress_result *out) 
         sizeof log, len_ms, poll, &ur.kernel_ns);
     out->gap_ns += (now_ns() - ts) - (ur.kernel_ns - kernel_before);
     if (lrc != GSB_OK) {
-      ur.status = lrc;
-      rc = lrc;
-      wedged = lrc == GSB_ERR_TIMEOUT;
+      ur.status = rc = lrc;
       break;
     }
     for (uint32_t s = 0; s < GSB_STRESS_SETS_MAX; s++) {
       ur.set_iterations[s] += log.set_iterations[s];
       ur.iterations += log.set_iterations[s];
     }
-    ur.words_checked += log.words;
-    ur.mismatch_words += log.mismatch_words;
-    ur.mismatch_bits += log.mismatch_bits;
     if (log.mismatch_words && out->first_mismatch_slice == UINT32_MAX) {
       out->first_mismatch_slice = i;
       out->first_mismatch_ms = (now_ns() - t0) / 1000000ull;
     }
-    for (int w = 0; w < GSB_SM_MAX / 32; w++) {
-      out->covered[w] = i == 0 ? log.covered[w] : out->covered[w] & log.covered[w];
-      out->faulty[w] |= log.faulty[w];
-    }
+    uint32_t covered[GSB_SM_MAX / 32] = {0};
+    fold_log(log, &ur, out, covered);
+    for (int w = 0; w < GSB_SM_MAX / 32; w++) out->covered[w] = i == 0 ? covered[w] : out->covered[w] & covered[w];
     for (uint32_t sm = 0; sm < GSB_SM_MAX; sm++) sm_iters[sm] += log.sm_iterations[sm];
-    const uint32_t got = log.count < GSB_SM_RECORDS ? log.count : GSB_SM_RECORDS;
-    for (uint32_t r = 0; r < got && out->n_records < GSB_SM_RECORDS; r++) out->records[out->n_records++] = log.rec[r];
   }
   if (out->slices) sampler.end();
   for (gsb_stress_unit_result &ur : out->unit) {
@@ -2472,8 +2425,7 @@ int stress_locked(Device *d, const gsb_stress_cfg *cfg, gsb_stress_result *out) 
     if (first || sm_iters[sm] > out->sm_iterations_max) out->sm_iterations_max = sm_iters[sm];
     first = false;
   }
-  if (wedged) d->sm_kept = buf;  // given back once the stream has drained
-  else if (buf) cudaFree(buf);
+  buf.release();
   out->wall_ns = now_ns() - t0;
   out->status = rc;
   return rc;
@@ -2504,12 +2456,9 @@ int cluster_probe_locked(Device *d, const gsb_cluster_cfg *cfg, gsb_cluster_resu
   out->sm_count = d->sm_count;
   int rc = ensure_ready(d);
   if (!rc) rc = sm_drain_kept_locked(d);
-  if (rc) return out->status = rc;
   int smem = 0;
-  if (cudaDeviceGetAttribute(&smem, cudaDevAttrMaxSharedMemoryPerBlockOptin, d->ordinal) != cudaSuccess) {
-    set_error("querying the shared-memory opt-in maximum of %s", d->uuid);
-    return out->status = GSB_ERR_DRIVER;
-  }
+  if (!rc) rc = smem_optin_locked(d, &smem);
+  if (rc) return out->status = rc;
   out->smem_bytes = (uint32_t)smem;
   for (uint32_t k = 0; k < GSB_CLUSTER_SIZES; k++) {
     const uint32_t n = 2u << k;
@@ -2524,23 +2473,14 @@ int cluster_probe_locked(Device *d, const gsb_cluster_cfg *cfg, gsb_cluster_resu
   }
   // the defaults: n = 2 (most likely the two SMs of a TPC) and the largest of 16 and 8 that can be scheduled (a GPC)
   out->sizes = cfg->sizes ? cfg->sizes : 1u | (out->max_clusters[3] ? 8u : out->max_clusters[2] ? 4u : 0u);
-  if (!cfg->seed) d->cluster_seed++;
-  out->seed = cfg->seed ? cfg->seed : 0x434C0000u + d->cluster_seed;  // fresh per probe
+  out->seed = seed_or_fresh(cfg->seed, 0x434C0000u, &d->cluster.seed);
   out->seed_expect = cfg->seed_expect ? cfg->seed_expect : out->seed;
-  Device::ClusterHook hooks[GSB_CLUSTER_PATHS];
-  {
-    std::lock_guard<std::mutex> lk(d->smu);
-    for (uint32_t p = 0; p < GSB_CLUSTER_PATHS; p++) {
-      hooks[p] = d->cluster_hook[p];
-      d->cluster_hook[p] = Device::ClusterHook{};
-    }
-  }
+  auto hooks = take_hooks(d, &d->cluster.hooks);
   // one transient buffer: the launch log, then the multicast source (n segments; at most the area of one CTA)
   const size_t log_bytes = (sizeof(gsb_cluster_log) + 255) / 256 * 256;
   const size_t src_bytes = 16ull * gsb_cluster_area_words((uint32_t)smem);
-  void *buf = nullptr;
-  rc = sm_alloc_locked(d, "SM-to-SM probe", log_bytes + src_bytes, &buf);
-  bool wedged = false;
+  SmBuffer buf(d, rc);
+  rc = buf.alloc("SM-to-SM probe", log_bytes + src_bytes);
   std::vector<uint32_t> src_words;
   for (uint32_t k = 0; k < GSB_CLUSTER_SIZES && rc == GSB_OK; k++) {
     if (!(out->sizes >> k & 1u)) continue;
@@ -2555,8 +2495,8 @@ int cluster_probe_locked(Device *d, const gsb_cluster_cfg *cfg, gsb_cluster_resu
       gsb_cluster_run &run = out->run[p][k];
       gsb_cluster_args a;
       memset(&a, 0, sizeof a);
-      a.log = static_cast<gsb_cluster_log *>(buf);
-      a.mc_src = static_cast<char *>(buf) + log_bytes;
+      a.log = static_cast<gsb_cluster_log *>(buf.p);
+      a.mc_src = static_cast<char *>(buf.p) + log_bytes;
       a.seed = out->seed;
       a.seed_expect = out->seed_expect;
       a.smem_bytes = (uint32_t)smem;
@@ -2590,68 +2530,29 @@ int cluster_probe_locked(Device *d, const gsb_cluster_cfg *cfg, gsb_cluster_resu
         gsb_cluster_log log;
         const int lrc = cluster_launch_locked(d, p, n, out->max_clusters[k], a, &log, &run.kernel_ns);
         if (lrc != GSB_OK) {
-          run.status = lrc;
-          rc = lrc;
-          wedged = lrc == GSB_ERR_TIMEOUT;
+          run.status = rc = lrc;
           break;
         }
-        run.words_checked += log.words;
-        run.mismatch_words += log.mismatch_words;
-        run.mismatch_bits += log.mismatch_bits;
         run.timeouts += log.timeouts;
-        for (int i = 0; i < GSB_CLUSTER_SM_MAX / 32; i++) {
-          covered[i] |= log.covered[i];
-          out->covered[i] |= log.covered[i];
-          out->faulty[i] |= log.faulty[i];
-        }
-        const uint32_t got = log.count < GSB_CLUSTER_RECORDS ? log.count : GSB_CLUSTER_RECORDS;
-        for (uint32_t i = 0; i < got && out->n_records < GSB_CLUSTER_RECORDS; i++)
-          out->records[out->n_records++] = log.rec[i];
+        fold_log(log, &run, out, covered);
       }
       run.sms_covered = popcount_bitmap(covered);
+      for (int i = 0; i < GSB_CLUSTER_SM_MAX / 32; i++) out->covered[i] |= covered[i];
     }
   }
-  if (wedged) d->sm_kept = buf;  // given back once the stream has drained
-  else if (buf) cudaFree(buf);
+  buf.release();
   out->wall_ns = now_ns() - t0;
   out->status = rc;
-  {
-    std::lock_guard<std::mutex> lk(d->smu);
-    gsb_cluster_stats &st = d->cluster_stats;
-    st.probes++;
-    bool ran = false, short_cover = false;
-    for (uint32_t p = 0; p < GSB_CLUSTER_PATHS; p++)
-      for (uint32_t k = 0; k < GSB_CLUSTER_SIZES; k++) {
-        const gsb_cluster_run &run = out->run[p][k];
-        ran = ran || run.launches != 0;
-        short_cover = short_cover || (run.launches != 0 && run.status == GSB_OK && run.sms_covered < out->expect_covered[k]);
-      }
-    if (!ran) st.skipped++;  // no launch ran: nothing was learnt about the network
-    if (short_cover) st.incomplete++;
-    if (gsb_cluster_conditions(out)) st.faults++;
-    st.last = *out;
-  }
+  bool ran = false, short_cover = false;
+  for (uint32_t p = 0; p < GSB_CLUSTER_PATHS; p++)
+    for (uint32_t k = 0; k < GSB_CLUSTER_SIZES; k++) {
+      const gsb_cluster_run &run = out->run[p][k];
+      ran = ran || run.launches != 0;
+      short_cover = short_cover || (run.launches != 0 && run.status == GSB_OK && run.sms_covered < out->expect_covered[k]);
+    }
+  count_probe(d, &d->cluster.stats, *out, ran, gsb_cluster_conditions(out),
+              short_cover ? &d->cluster.stats.incomplete : nullptr);
   return rc;
-}
-
-// Raise every condition of `r` this device has not raised yet this health session (one event per condition).
-void raise_cluster_conditions(Device *d, const gsb_cluster_result &r) {
-  uint32_t fresh;
-  {
-    std::lock_guard<std::mutex> lk(d->smu);
-    fresh = gsb_cluster_conditions(&r) & ~d->cluster_raised;
-    d->cluster_raised |= fresh;
-  }
-  for (uint32_t bit = 1; fresh; bit <<= 1) {
-    if (!(fresh & bit)) continue;
-    fresh &= ~bit;
-    gsb_event ev;
-    memset(&ev, 0, sizeof ev);
-    snprintf(ev.uuid, sizeof ev.uuid, "%s", d->uuid);
-    ev.etype = GSB_EVENT_CLUSTER;
-    ev.edata = bit;
-    push_event(ev);
-  }
 }
 
 // ------------------------------------------------------------------ L2 atomic health (gsb_atomic_probe)
@@ -2706,30 +2607,19 @@ int atomic_probe_locked(Device *d, const gsb_atomic_cfg *cfg, gsb_atomic_result 
     return out->status = GSB_ERR_INVALID_ARGUMENT;
   }
   int smem = 0;
-  if (cudaDeviceGetAttribute(&smem, cudaDevAttrMaxSharedMemoryPerBlockOptin, d->ordinal) != cudaSuccess) {
-    set_error("querying the shared-memory opt-in maximum of %s", d->uuid);
-    return out->status = GSB_ERR_DRIVER;
-  }
-  if (!cfg->seed) d->atomic_seed++;
-  out->seed = cfg->seed ? cfg->seed : 0x41540000u + d->atomic_seed;  // fresh per probe
+  if ((rc = smem_optin_locked(d, &smem))) return out->status = rc;
+  out->seed = seed_or_fresh(cfg->seed, 0x41540000u, &d->atomic.seed);
   out->seed_expect = cfg->seed_expect ? cfg->seed_expect : out->seed;
-  Device::AtomicHook hooks[GSB_ATOMIC_OPS];
-  {
-    std::lock_guard<std::mutex> lk(d->smu);
-    for (uint32_t o = 0; o < GSB_ATOMIC_OPS; o++) {
-      hooks[o] = d->atomic_hook[o];
-      d->atomic_hook[o] = Device::AtomicHook{};
-    }
-  }
+  const auto hooks = take_hooks(d, &d->atomic.hooks);
   // one transient buffer: the run and check logs, the words, the expected words, the ticket slots
   const uint32_t ctas = d->sm_count;
   const size_t slot_words = (size_t)GSB_ATOMIC_HOT_WORDS * gsb_atomic_hot_count(GSB_ATOMIC_OP_TICKET, ctas);
   const size_t off_words = 2 * kAtomicLogBytes, off_expect = off_words + GSB_ATOMIC_BYTES;
   const size_t off_slots = off_expect + GSB_ATOMIC_BYTES, bytes = off_slots + 4 * slot_words;
-  void *buf = nullptr;
-  rc = sm_alloc_locked(d, "L2 atomic probe", bytes, &buf);
-  char *base = static_cast<char *>(buf);
-  bool wedged = false, first = true;
+  SmBuffer buf(d, rc);
+  rc = buf.alloc("L2 atomic probe", bytes);
+  char *base = static_cast<char *>(buf.p);
+  bool first = true;
   std::vector<unsigned char> expect(GSB_ATOMIC_BYTES);
   std::vector<uint32_t> slots;
   for (uint32_t op = 0; op < GSB_ATOMIC_OPS && rc == GSB_OK; op++) {
@@ -2797,7 +2687,6 @@ int atomic_probe_locked(Device *d, const gsb_atomic_cfg *cfg, gsb_atomic_result 
       }
       if (lrc != GSB_OK) {
         run.status = rc = lrc;
-        wedged = lrc == GSB_ERR_TIMEOUT;
         break;
       }
       if (rl.skipped_cta) run.hook_cta = rl.skipped_cta - 1u;
@@ -2818,45 +2707,112 @@ int atomic_probe_locked(Device *d, const gsb_atomic_cfg *cfg, gsb_atomic_result 
     for (int i = 0; i < GSB_ATOMIC_SM_MAX / 32; i++) out->covered[i] = first ? covered[i] : out->covered[i] & covered[i];
     first = false;
   }
-  if (wedged) d->sm_kept = buf;  // given back once the stream has drained
-  else if (buf) cudaFree(buf);
+  buf.release();
   out->wall_ns = now_ns() - t0;
   out->status = rc;
-  {
-    std::lock_guard<std::mutex> lk(d->smu);
-    gsb_atomic_stats &st = d->atomic_stats;
-    st.probes++;
-    bool ran = false, short_cover = false;
-    for (const gsb_atomic_run &run : out->run) {
-      ran = ran || run.launches != 0;
-      short_cover = short_cover || (run.launches != 0 && run.status == GSB_OK && run.sms_covered < out->sm_count);
-    }
-    if (!ran) st.skipped++;  // no launch ran: nothing was learnt about the atomics
-    if (short_cover) st.incomplete++;
-    if (gsb_atomic_conditions(out)) st.faults++;
-    st.last = *out;
+  bool ran = false, short_cover = false;
+  for (const gsb_atomic_run &run : out->run) {
+    ran = ran || run.launches != 0;
+    short_cover = short_cover || (run.launches != 0 && run.status == GSB_OK && run.sms_covered < out->sm_count);
   }
+  count_probe(d, &d->atomic.stats, *out, ran, gsb_atomic_conditions(out),
+              short_cover ? &d->atomic.stats.incomplete : nullptr);
   return rc;
 }
 
-// Raise every condition of `r` this device has not raised yet this health session (one event per condition).
-void raise_atomic_conditions(Device *d, const gsb_atomic_result &r) {
-  uint32_t fresh;
-  {
-    std::lock_guard<std::mutex> lk(d->smu);
-    fresh = gsb_atomic_conditions(&r) & ~d->atomic_raised;
-    d->atomic_raised |= fresh;
-  }
-  for (uint32_t bit = 1; fresh; bit <<= 1) {
-    if (!(fresh & bit)) continue;
-    fresh &= ~bit;
-    gsb_event ev;
-    memset(&ev, 0, sizeof ev);
-    snprintf(ev.uuid, sizeof ev.uuid, "%s", d->uuid);
-    ev.etype = GSB_EVENT_ATOMIC;
-    ev.edata = bit;
-    push_event(ev);
-  }
+// ------------------------------------------------------------------ the periodic checks, described once
+
+template <typename Run>
+struct RunTypes;
+template <typename C, typename R>
+struct RunTypes<int (*)(Device *, const C *, R *)> {
+  using Cfg = C;
+  using Result = R;
+};
+
+// One check the prober runs every Nth cycle: its cadence option, the event its conditions raise, where a device keeps
+// its state, its run under d->mu and the conditions of a result.
+template <uint32_t kOption, uint64_t kEvent, auto kState, auto kRun, auto kConditions>
+struct Check {
+  static constexpr uint32_t option = kOption;
+  static constexpr uint64_t event = kEvent;
+  using Cfg = typename RunTypes<decltype(kRun)>::Cfg;
+  using Result = typename RunTypes<decltype(kRun)>::Result;
+  static auto &state(Device *d) { return d->*kState; }
+  static int run(Device *d, const Cfg *cfg, Result *out) { return kRun(d, cfg, out); }
+  static uint32_t conditions(const Result *r) { return kConditions(r); }
+};
+using LinkCheck = Check<GSB_OPT_LINK_PROBE_EVERY_CYCLES, GSB_EVENT_LINK, &Device::link, &link_probe_locked, &gsb_link_conditions>;
+using CopyCheck = Check<GSB_OPT_COPY_PROBE_EVERY_CYCLES, GSB_EVENT_COPY, &Device::copy, &copy_probe_locked, &gsb_copy_conditions>;
+using SmCheck = Check<GSB_OPT_SM_PROBE_EVERY_CYCLES, GSB_EVENT_SM, &Device::sm, &sm_probe_locked, &gsb_sm_conditions>;
+using ClusterCheck = Check<GSB_OPT_CLUSTER_PROBE_EVERY_CYCLES, GSB_EVENT_CLUSTER, &Device::cluster,
+                           &cluster_probe_locked, &gsb_cluster_conditions>;
+using AtomicCheck = Check<GSB_OPT_ATOMIC_PROBE_EVERY_CYCLES, GSB_EVENT_ATOMIC, &Device::atomic, &atomic_probe_locked,
+                          &gsb_atomic_conditions>;
+// in the order the prober runs them when several are due after the same cycle; G.check_every follows it
+using Checks = std::tuple<LinkCheck, CopyCheck, SmCheck, ClusterCheck, AtomicCheck>;
+static_assert(std::tuple_size<Checks>::value == std::extent<decltype(G.check_every)>::value, "one cadence per check");
+
+// f(check, its place in Checks) for every periodic check, in order
+template <typename F, size_t... I>
+void for_each_check(F &&f, std::index_sequence<I...>) {
+  (f(std::tuple_element_t<I, Checks>{}, I), ...);
+}
+template <typename F>
+void for_each_check(F &&f) {
+  for_each_check(f, std::make_index_sequence<std::tuple_size<Checks>::value>{});
+}
+
+// The cadence a GSB_OPT_*_PROBE_EVERY_CYCLES key sets, or null for any other key.
+std::atomic<uint64_t> *check_every_of(uint32_t key) {
+  std::atomic<uint64_t> *every = nullptr;
+  for_each_check([&](auto check, size_t i) {
+    if (decltype(check)::option == key) every = &G.check_every[i];
+  });
+  return every;
+}
+
+// The body of a probe entry point: `pre` (if any) may refuse the arguments before any device is touched; the run then
+// holds d->mu from start to end, so a prober cycle waits for it.
+template <typename Cfg, typename Result, typename Pre>
+int probe_entry(uint32_t idx, const Cfg *cfg, Result *out, int (*run)(Device *, const Cfg *, Result *), Pre pre) {
+  std::shared_lock<std::shared_mutex> api_lk(G.api_mu);
+  if (!cfg || !out) return GSB_ERR_INVALID_ARGUMENT;
+  memset(out, 0, sizeof *out);
+  const int refused = pre(cfg, out);
+  if (refused) return out->status = refused;
+  Device *d = device_at(idx);
+  if (!d) return out->status = G.inited ? GSB_ERR_NO_DEVICE : GSB_ERR_NOT_INITIALIZED;
+  std::lock_guard<std::mutex> lk(d->mu);
+  return run(d, cfg, out);
+}
+template <typename Cfg, typename Result>
+int probe_entry(uint32_t idx, const Cfg *cfg, Result *out, int (*run)(Device *, const Cfg *, Result *)) {
+  return probe_entry(idx, cfg, out, run, [](const Cfg *, Result *) { return GSB_OK; });
+}
+
+// The body of a gsb_*_stats_get: a copy, under smu, of the statistics `stats` finds in the device.
+template <typename Stats, typename Find>
+int stats_entry(uint32_t idx, Stats *out, Find stats) {
+  std::shared_lock<std::shared_mutex> api_lk(G.api_mu);
+  if (!out) return GSB_ERR_INVALID_ARGUMENT;
+  Device *d = device_at(idx);
+  if (!d) return G.inited ? GSB_ERR_NO_DEVICE : GSB_ERR_NOT_INITIALIZED;
+  std::lock_guard<std::mutex> lk(d->smu);
+  *out = *stats(d);
+  return GSB_OK;
+}
+
+// One periodic check of device idx on default settings, and an event for every condition it finds for the first time
+// this health session.
+template <typename C>
+void run_check(uint32_t idx) {
+  typename C::Cfg cfg;
+  memset(&cfg, 0, sizeof cfg);
+  typename C::Result r;
+  probe_entry(idx, &cfg, &r, &C::run);
+  Device *d = G.devs[idx].get();
+  raise_conditions(d, C::event, &C::state(d).raised, [&] { return C::conditions(&r); });
 }
 
 }  // namespace
@@ -3246,12 +3202,13 @@ int gsb_set_option(uint32_t key, uint64_t value) {
       if (value > 1) return GSB_ERR_INVALID_ARGUMENT;
       G.ecc_health = value;
       return GSB_OK;
-    case GSB_OPT_LINK_PROBE_EVERY_CYCLES: G.link_every = value; return GSB_OK;
-    case GSB_OPT_COPY_PROBE_EVERY_CYCLES: G.copy_every = value; return GSB_OK;
-    case GSB_OPT_SM_PROBE_EVERY_CYCLES: G.sm_every = value; return GSB_OK;
-    case GSB_OPT_CLUSTER_PROBE_EVERY_CYCLES: G.cluster_every = value; return GSB_OK;
-    case GSB_OPT_ATOMIC_PROBE_EVERY_CYCLES: G.atomic_every = value; return GSB_OK;
-    default: set_error("unknown option %u", key); return GSB_ERR_INVALID_ARGUMENT;
+    default:
+      if (std::atomic<uint64_t> *every = check_every_of(key)) {
+        *every = value;
+        return GSB_OK;
+      }
+      set_error("unknown option %u", key);
+      return GSB_ERR_INVALID_ARGUMENT;
   }
 }
 
@@ -3265,12 +3222,13 @@ int gsb_get_option(uint32_t key, uint64_t *value) {
     case GSB_OPT_TRANSIENT_KEEP_FREE_BYTES: *value = G.transient_keep_free; return GSB_OK;
     case GSB_OPT_SWEEP_EVERY_CYCLES: *value = G.sweep_every; return GSB_OK;
     case GSB_OPT_ECC_HEALTH: *value = G.ecc_health; return GSB_OK;
-    case GSB_OPT_LINK_PROBE_EVERY_CYCLES: *value = G.link_every; return GSB_OK;
-    case GSB_OPT_COPY_PROBE_EVERY_CYCLES: *value = G.copy_every; return GSB_OK;
-    case GSB_OPT_SM_PROBE_EVERY_CYCLES: *value = G.sm_every; return GSB_OK;
-    case GSB_OPT_CLUSTER_PROBE_EVERY_CYCLES: *value = G.cluster_every; return GSB_OK;
-    case GSB_OPT_ATOMIC_PROBE_EVERY_CYCLES: *value = G.atomic_every; return GSB_OK;
-    default: set_error("unknown option %u", key); return GSB_ERR_INVALID_ARGUMENT;
+    default:
+      if (const std::atomic<uint64_t> *every = check_every_of(key)) {
+        *value = *every;
+        return GSB_OK;
+      }
+      set_error("unknown option %u", key);
+      return GSB_ERR_INVALID_ARGUMENT;
   }
 }
 
@@ -3354,23 +3312,11 @@ int gsb_ecc_status_get(uint32_t idx, gsb_ecc_status *out) {
 }
 
 int gsb_ecc_stats_get(uint32_t idx, gsb_ecc_stats *out) {
-  std::shared_lock<std::shared_mutex> api_lk(G.api_mu);
-  if (!out) return GSB_ERR_INVALID_ARGUMENT;
-  Device *d = device_at(idx);
-  if (!d) return G.inited ? GSB_ERR_NO_DEVICE : GSB_ERR_NOT_INITIALIZED;
-  std::lock_guard<std::mutex> lk(d->smu);
-  *out = d->ecc_stats;
-  return GSB_OK;
+  return stats_entry(idx, out, [](Device *d) { return &d->ecc_stats; });
 }
 
 int gsb_memtest(uint32_t idx, const gsb_memtest_cfg *cfg, gsb_memtest_result *out) {
-  std::shared_lock<std::shared_mutex> api_lk(G.api_mu);
-  if (!cfg || !out) return GSB_ERR_INVALID_ARGUMENT;
-  memset(out, 0, sizeof *out);
-  Device *d = device_at(idx);
-  if (!d) return out->status = G.inited ? GSB_ERR_NO_DEVICE : GSB_ERR_NOT_INITIALIZED;
-  std::lock_guard<std::mutex> lk(d->mu);  // the whole run: a prober cycle waits
-  return memtest_locked(d, cfg, out);
+  return probe_entry(idx, cfg, out, &memtest_locked);
 }
 
 int gsb_test_ecc_override(uint32_t idx, const gsb_ecc_status *st) {
@@ -3384,13 +3330,7 @@ int gsb_test_ecc_override(uint32_t idx, const gsb_ecc_status *st) {
 }
 
 int gsb_link_probe(uint32_t idx, const gsb_link_cfg *cfg, gsb_link_result *out) {
-  std::shared_lock<std::shared_mutex> api_lk(G.api_mu);
-  if (!cfg || !out) return GSB_ERR_INVALID_ARGUMENT;
-  memset(out, 0, sizeof *out);
-  Device *d = device_at(idx);
-  if (!d) return out->status = G.inited ? GSB_ERR_NO_DEVICE : GSB_ERR_NOT_INITIALIZED;
-  std::lock_guard<std::mutex> lk(d->mu);  // the whole probe: a prober cycle waits
-  return link_probe_locked(d, cfg, out);
+  return probe_entry(idx, cfg, out, &LinkCheck::run);
 }
 
 int gsb_link_status_get(uint32_t idx, gsb_link_status *out) {
@@ -3403,13 +3343,7 @@ int gsb_link_status_get(uint32_t idx, gsb_link_status *out) {
 }
 
 int gsb_link_stats_get(uint32_t idx, gsb_link_stats *out) {
-  std::shared_lock<std::shared_mutex> api_lk(G.api_mu);
-  if (!out) return GSB_ERR_INVALID_ARGUMENT;
-  Device *d = device_at(idx);
-  if (!d) return G.inited ? GSB_ERR_NO_DEVICE : GSB_ERR_NOT_INITIALIZED;
-  std::lock_guard<std::mutex> lk(d->smu);
-  *out = d->link_stats;
-  return GSB_OK;
+  return stats_entry(idx, out, [](Device *d) { return &d->link.stats; });
 }
 
 int gsb_test_link_override(uint32_t idx, const gsb_link_status *st) {
@@ -3432,28 +3366,16 @@ int gsb_test_link_corrupt(uint32_t idx, uint32_t phase, uint64_t offset, const u
   c.phase = phase;
   c.offset = offset;
   memcpy(c.xr, xr, sizeof c.xr);
-  d->link_corrupt.push_back(c);
+  d->link.hooks.push_back(c);
   return GSB_OK;
 }
 
 int gsb_copy_probe(uint32_t idx, const gsb_copy_cfg *cfg, gsb_copy_result *out) {
-  std::shared_lock<std::shared_mutex> api_lk(G.api_mu);
-  if (!cfg || !out) return GSB_ERR_INVALID_ARGUMENT;
-  memset(out, 0, sizeof *out);
-  Device *d = device_at(idx);
-  if (!d) return out->status = G.inited ? GSB_ERR_NO_DEVICE : GSB_ERR_NOT_INITIALIZED;
-  std::lock_guard<std::mutex> lk(d->mu);  // the whole probe: a prober cycle waits
-  return copy_probe_locked(d, cfg, out);
+  return probe_entry(idx, cfg, out, &CopyCheck::run);
 }
 
 int gsb_copy_stats_get(uint32_t idx, gsb_copy_stats *out) {
-  std::shared_lock<std::shared_mutex> api_lk(G.api_mu);
-  if (!out) return GSB_ERR_INVALID_ARGUMENT;
-  Device *d = device_at(idx);
-  if (!d) return G.inited ? GSB_ERR_NO_DEVICE : GSB_ERR_NOT_INITIALIZED;
-  std::lock_guard<std::mutex> lk(d->smu);
-  *out = d->copy_stats;
-  return GSB_OK;
+  return stats_entry(idx, out, [](Device *d) { return &d->copy.stats; });
 }
 
 int gsb_test_copy_corrupt(uint32_t idx, uint32_t op, uint64_t offset, const uint32_t xr[4]) {
@@ -3466,7 +3388,7 @@ int gsb_test_copy_corrupt(uint32_t idx, uint32_t op, uint64_t offset, const uint
   c.dir = op - GSB_OP_COPY_H2D;
   c.offset = offset;
   memcpy(c.xr, xr, sizeof c.xr);
-  d->copy_corrupt.push_back(c);
+  d->copy.hooks.corrupt.push_back(c);
   return GSB_OK;
 }
 
@@ -3476,28 +3398,16 @@ int gsb_test_copy_skip(uint32_t idx, uint32_t op) {
   Device *d = device_at(idx);
   if (!d) return G.inited ? GSB_ERR_NO_DEVICE : GSB_ERR_NOT_INITIALIZED;
   std::lock_guard<std::mutex> lk(d->smu);
-  d->copy_skip |= 1u << (op - GSB_OP_COPY_H2D);
+  d->copy.hooks.skip |= 1u << (op - GSB_OP_COPY_H2D);
   return GSB_OK;
 }
 
 int gsb_sm_probe(uint32_t idx, const gsb_sm_cfg *cfg, gsb_sm_result *out) {
-  std::shared_lock<std::shared_mutex> api_lk(G.api_mu);
-  if (!cfg || !out) return GSB_ERR_INVALID_ARGUMENT;
-  memset(out, 0, sizeof *out);
-  Device *d = device_at(idx);
-  if (!d) return out->status = G.inited ? GSB_ERR_NO_DEVICE : GSB_ERR_NOT_INITIALIZED;
-  std::lock_guard<std::mutex> lk(d->mu);  // the whole probe: a prober cycle waits
-  return sm_probe_locked(d, cfg, out);
+  return probe_entry(idx, cfg, out, &SmCheck::run);
 }
 
 int gsb_sm_stats_get(uint32_t idx, gsb_sm_stats *out) {
-  std::shared_lock<std::shared_mutex> api_lk(G.api_mu);
-  if (!out) return GSB_ERR_INVALID_ARGUMENT;
-  Device *d = device_at(idx);
-  if (!d) return G.inited ? GSB_ERR_NO_DEVICE : GSB_ERR_NOT_INITIALIZED;
-  std::lock_guard<std::mutex> lk(d->smu);
-  *out = d->sm_stats;
-  return GSB_OK;
+  return stats_entry(idx, out, [](Device *d) { return &d->sm.stats; });
 }
 
 int gsb_test_sm_corrupt(uint32_t idx, uint32_t smid, uint32_t unit, uint32_t index, uint64_t xr) {
@@ -3508,7 +3418,7 @@ int gsb_test_sm_corrupt(uint32_t idx, uint32_t smid, uint32_t unit, uint32_t ind
   Device *d = device_at(idx);
   if (!d) return G.inited ? GSB_ERR_NO_DEVICE : GSB_ERR_NOT_INITIALIZED;
   std::lock_guard<std::mutex> lk(d->smu);
-  Device::SmCorrupt &c = d->sm_corrupt[unit];
+  Device::SmCorrupt &c = d->sm.hooks.corrupt[unit];
   c.armed = true;
   c.smid = smid;
   c.index = index;
@@ -3547,22 +3457,18 @@ int gsb_test_sm_operands(uint32_t idx, uint32_t unit, const int32_t *a, const in
   Device *d = device_at(idx);
   if (!d) return G.inited ? GSB_ERR_NO_DEVICE : GSB_ERR_NOT_INITIALIZED;
   std::lock_guard<std::mutex> lk(d->smu);
-  d->sm_operands[unit].swap(t);
+  d->sm.hooks.operands[unit].swap(t);
   return GSB_OK;
 }
 
 int gsb_sm_stress(uint32_t idx, const gsb_stress_cfg *cfg, gsb_stress_result *out) {
-  std::shared_lock<std::shared_mutex> api_lk(G.api_mu);
-  if (!cfg || !out) return GSB_ERR_INVALID_ARGUMENT;
-  memset(out, 0, sizeof *out);
-  out->first_mismatch_slice = UINT32_MAX;
-  if ((cfg->units & ~GSB_STRESS_UNIT_MASK) || cfg->duration_ms == 0 || cfg->duration_ms > GSB_STRESS_DURATION_MAX_MS ||
-      cfg->slice_ms > GSB_STRESS_SLICE_MAX_MS)
-    return out->status = GSB_ERR_INVALID_ARGUMENT;  // refused before any device is touched
-  Device *d = device_at(idx);
-  if (!d) return out->status = G.inited ? GSB_ERR_NO_DEVICE : GSB_ERR_NOT_INITIALIZED;
-  std::lock_guard<std::mutex> lk(d->mu);  // the whole run: a prober cycle waits
-  return stress_locked(d, cfg, out);
+  return probe_entry(idx, cfg, out, &stress_locked, [](const gsb_stress_cfg *cfg, gsb_stress_result *out) {
+    out->first_mismatch_slice = UINT32_MAX;
+    // refused here, before any device is touched
+    const bool bad = (cfg->units & ~GSB_STRESS_UNIT_MASK) || cfg->duration_ms == 0 ||
+                     cfg->duration_ms > GSB_STRESS_DURATION_MAX_MS || cfg->slice_ms > GSB_STRESS_SLICE_MAX_MS;
+    return bad ? GSB_ERR_INVALID_ARGUMENT : GSB_OK;
+  });
 }
 
 int gsb_test_stress_corrupt(uint32_t idx, uint32_t smid, uint32_t unit, uint32_t index, uint32_t xr, uint32_t slice) {
@@ -3578,23 +3484,11 @@ int gsb_test_stress_corrupt(uint32_t idx, uint32_t smid, uint32_t unit, uint32_t
 }
 
 int gsb_cluster_probe(uint32_t idx, const gsb_cluster_cfg *cfg, gsb_cluster_result *out) {
-  std::shared_lock<std::shared_mutex> api_lk(G.api_mu);
-  if (!cfg || !out) return GSB_ERR_INVALID_ARGUMENT;
-  memset(out, 0, sizeof *out);
-  Device *d = device_at(idx);
-  if (!d) return out->status = G.inited ? GSB_ERR_NO_DEVICE : GSB_ERR_NOT_INITIALIZED;
-  std::lock_guard<std::mutex> lk(d->mu);  // the whole probe: a prober cycle waits
-  return cluster_probe_locked(d, cfg, out);
+  return probe_entry(idx, cfg, out, &ClusterCheck::run);
 }
 
 int gsb_cluster_stats_get(uint32_t idx, gsb_cluster_stats *out) {
-  std::shared_lock<std::shared_mutex> api_lk(G.api_mu);
-  if (!out) return GSB_ERR_INVALID_ARGUMENT;
-  Device *d = device_at(idx);
-  if (!d) return G.inited ? GSB_ERR_NO_DEVICE : GSB_ERR_NOT_INITIALIZED;
-  std::lock_guard<std::mutex> lk(d->smu);
-  *out = d->cluster_stats;
-  return GSB_OK;
+  return stats_entry(idx, out, [](Device *d) { return &d->cluster.stats; });
 }
 
 int gsb_test_cluster_corrupt(uint32_t idx, uint32_t smid, uint32_t path, uint32_t index, uint64_t xr) {
@@ -3604,7 +3498,7 @@ int gsb_test_cluster_corrupt(uint32_t idx, uint32_t smid, uint32_t path, uint32_
   Device *d = device_at(idx);
   if (!d) return G.inited ? GSB_ERR_NO_DEVICE : GSB_ERR_NOT_INITIALIZED;
   std::lock_guard<std::mutex> lk(d->smu);
-  Device::ClusterHook &h = d->cluster_hook[path];
+  Device::ClusterHook &h = d->cluster.hooks[path];
   h.corrupt = true;
   h.corrupt_smid = smid;
   h.index = index;
@@ -3618,30 +3512,18 @@ int gsb_test_cluster_skip(uint32_t idx, uint32_t smid, uint32_t path) {
   Device *d = device_at(idx);
   if (!d) return G.inited ? GSB_ERR_NO_DEVICE : GSB_ERR_NOT_INITIALIZED;
   std::lock_guard<std::mutex> lk(d->smu);
-  Device::ClusterHook &h = d->cluster_hook[path];
+  Device::ClusterHook &h = d->cluster.hooks[path];
   h.skip = true;
   h.skip_smid = smid;
   return GSB_OK;
 }
 
 int gsb_atomic_probe(uint32_t idx, const gsb_atomic_cfg *cfg, gsb_atomic_result *out) {
-  std::shared_lock<std::shared_mutex> api_lk(G.api_mu);
-  if (!cfg || !out) return GSB_ERR_INVALID_ARGUMENT;
-  memset(out, 0, sizeof *out);
-  Device *d = device_at(idx);
-  if (!d) return out->status = G.inited ? GSB_ERR_NO_DEVICE : GSB_ERR_NOT_INITIALIZED;
-  std::lock_guard<std::mutex> lk(d->mu);  // the whole probe: a prober cycle waits
-  return atomic_probe_locked(d, cfg, out);
+  return probe_entry(idx, cfg, out, &AtomicCheck::run);
 }
 
 int gsb_atomic_stats_get(uint32_t idx, gsb_atomic_stats *out) {
-  std::shared_lock<std::shared_mutex> api_lk(G.api_mu);
-  if (!out) return GSB_ERR_INVALID_ARGUMENT;
-  Device *d = device_at(idx);
-  if (!d) return G.inited ? GSB_ERR_NO_DEVICE : GSB_ERR_NOT_INITIALIZED;
-  std::lock_guard<std::mutex> lk(d->smu);
-  *out = d->atomic_stats;
-  return GSB_OK;
+  return stats_entry(idx, out, [](Device *d) { return &d->atomic.stats; });
 }
 
 int gsb_test_atomic_corrupt(uint32_t idx, uint32_t op, uint32_t word, uint64_t xr) {
@@ -3651,7 +3533,7 @@ int gsb_test_atomic_corrupt(uint32_t idx, uint32_t op, uint32_t word, uint64_t x
   Device *d = device_at(idx);
   if (!d) return G.inited ? GSB_ERR_NO_DEVICE : GSB_ERR_NOT_INITIALIZED;
   std::lock_guard<std::mutex> lk(d->smu);
-  Device::AtomicHook &h = d->atomic_hook[op];
+  Device::AtomicHook &h = d->atomic.hooks[op];
   h.corrupt = true;
   h.word = word;
   h.xr = xr;
@@ -3664,7 +3546,7 @@ int gsb_test_atomic_skip(uint32_t idx, uint32_t smid, uint32_t op) {
   Device *d = device_at(idx);
   if (!d) return G.inited ? GSB_ERR_NO_DEVICE : GSB_ERR_NOT_INITIALIZED;
   std::lock_guard<std::mutex> lk(d->smu);
-  Device::AtomicHook &h = d->atomic_hook[op];
+  Device::AtomicHook &h = d->atomic.hooks[op];
   h.skip = true;
   h.skip_smid = smid;
   return GSB_OK;
@@ -3853,16 +3735,11 @@ int gsb_health_start(uint32_t probe_period_ms, uint64_t window_bytes) {
       d->ecc_raised = 0;
       d->ecc_baseline = ecc ? base : gsb_ecc_status{};
       if (ecc) d->ecc_stats.queries = 1;
-      d->link_stats = gsb_link_stats{};
-      d->link_raised = 0;
-      d->copy_stats = gsb_copy_stats{};
-      d->copy_raised = 0;
-      d->sm_stats = gsb_sm_stats{};
-      d->sm_raised = 0;
-      d->cluster_stats = gsb_cluster_stats{};
-      d->cluster_raised = 0;
-      d->atomic_stats = gsb_atomic_stats{};
-      d->atomic_raised = 0;
+      for_each_check([&](auto check, size_t) {
+        auto &state = decltype(check)::state(d.get());
+        state.stats = {};
+        state.raised = 0;
+      });
     }
     if (ecc) raise_ecc_conditions(d.get(), base);
   }
@@ -4040,51 +3917,12 @@ int gsb_health_start(uint32_t probe_period_ms, uint64_t window_bytes) {
               clean = 0;
             }
           }
-          // PCIe link health (opt-in): after the session's first cycle and every Nth one, outside gsb_cycle
-          const uint64_t link_every = G.link_every.load(std::memory_order_relaxed);
-          if (link_every && this_cycle % link_every == 0 && !G.health_stop.load()) {
-            gsb_link_cfg lc;
-            memset(&lc, 0, sizeof lc);
-            gsb_link_result lr;
-            gsb_link_probe(i, &lc, &lr);
-            raise_link_conditions(G.devs[i].get(), lr);
-          }
-          // copy-engine health (opt-in): likewise, after the link probe when both are due
-          const uint64_t copy_every = G.copy_every.load(std::memory_order_relaxed);
-          if (copy_every && this_cycle % copy_every == 0 && !G.health_stop.load()) {
-            gsb_copy_cfg cc;
-            memset(&cc, 0, sizeof cc);
-            gsb_copy_result cpr;
-            gsb_copy_probe(i, &cc, &cpr);
-            raise_copy_conditions(G.devs[i].get(), cpr);
-          }
-          // SM compute health (opt-in): likewise, after the link and copy probes when they are due
-          const uint64_t sm_every = G.sm_every.load(std::memory_order_relaxed);
-          if (sm_every && this_cycle % sm_every == 0 && !G.health_stop.load()) {
-            gsb_sm_cfg sc;
-            memset(&sc, 0, sizeof sc);
-            gsb_sm_result smr;
-            gsb_sm_probe(i, &sc, &smr);
-            raise_sm_conditions(G.devs[i].get(), smr);
-          }
-          // SM-to-SM health (opt-in): likewise, after the link, copy and SM probes when they are due
-          const uint64_t cluster_every = G.cluster_every.load(std::memory_order_relaxed);
-          if (cluster_every && this_cycle % cluster_every == 0 && !G.health_stop.load()) {
-            gsb_cluster_cfg kc;
-            memset(&kc, 0, sizeof kc);
-            gsb_cluster_result kr;
-            gsb_cluster_probe(i, &kc, &kr);
-            raise_cluster_conditions(G.devs[i].get(), kr);
-          }
-          // L2 atomic health (opt-in): likewise, after the link, copy, SM and SM-to-SM probes when they are due
-          const uint64_t atomic_every = G.atomic_every.load(std::memory_order_relaxed);
-          if (atomic_every && this_cycle % atomic_every == 0 && !G.health_stop.load()) {
-            gsb_atomic_cfg ac;
-            memset(&ac, 0, sizeof ac);
-            gsb_atomic_result ar;
-            gsb_atomic_probe(i, &ac, &ar);
-            raise_atomic_conditions(G.devs[i].get(), ar);
-          }
+          // the periodic checks (each opt-in): after the session's first cycle and every Nth one, outside gsb_cycle, in
+          // the order of Checks when several are due
+          for_each_check([&](auto check, size_t k) {
+            const uint64_t n = G.check_every[k].load(std::memory_order_relaxed);
+            if (n && this_cycle % n == 0 && !G.health_stop.load()) run_check<decltype(check)>(i);
+          });
           for (uint32_t slept = 0; slept < probe_period_ms && !G.health_stop.load(); slept += 10)
             std::this_thread::sleep_for(std::chrono::milliseconds(10));
         }

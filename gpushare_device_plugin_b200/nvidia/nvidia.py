@@ -118,69 +118,46 @@ def eccStatusLine(uuid: str) -> str:
     return device.ecc_status_text(st, uuid)
 
 
-def linkLine(uuid: str) -> str:
-    """gsb_link_text of GPU `uuid`'s most recent link probe; every reading "unknown" when there is none."""
-    r = LinkResult()
+@dataclass(frozen=True, eq=False)
+class Check:
+    """One periodic health check of the library (none is in the reference): what turns it on, what it raises and how
+    its most recent probe reads."""
+    option: int                          # GSB_OPT_*_PROBE_EVERY_CYCLES
+    event: int                           # GSB_EVENT_*
+    stats: Callable[[int], object]       # device.*_stats
+    text: Callable[[object, str], str]   # device.*_text
+    empty: Callable[[], object]          # the result of a probe that has not run
+    conditions: Dict[int, str]           # the name of each condition bit
+    label: str                           # in the warning
+    what: str                            # "<what> condition ?" stands for a condition without a name
+
+
+# in the order the library runs them, which is the order watchXIDs takes their cadences and logs them in
+CHECKS = (
+    Check(GSB_OPT_LINK_PROBE_EVERY_CYCLES, GSB_EVENT_LINK, device.link_stats, device.link_text, LinkResult,
+          LINK_CONDITION_NAMES, "PCIe link health", "link"),
+    Check(GSB_OPT_COPY_PROBE_EVERY_CYCLES, GSB_EVENT_COPY, device.copy_stats, device.copy_text, CopyResult,
+          COPY_CONDITION_NAMES, "copy-engine health", "copy"),
+    Check(GSB_OPT_SM_PROBE_EVERY_CYCLES, GSB_EVENT_SM, device.sm_stats, device.sm_text, SmResult,
+          SM_CONDITION_NAMES, "SM compute health", "SM"),
+    Check(GSB_OPT_CLUSTER_PROBE_EVERY_CYCLES, GSB_EVENT_CLUSTER, device.cluster_stats, device.cluster_text,
+          ClusterResult, CLUSTER_CONDITION_NAMES, "SM-to-SM health", "SM-to-SM"),
+    Check(GSB_OPT_ATOMIC_PROBE_EVERY_CYCLES, GSB_EVENT_ATOMIC, device.atomic_stats, device.atomic_text, AtomicResult,
+          ATOMIC_CONDITION_NAMES, "L2 atomic health", "L2 atomic"),
+)
+
+
+def checkLine(check: Check, uuid: str) -> str:
+    """The text of GPU `uuid`'s most recent probe of `check`; that of a probe that has not run when there is none."""
+    r = check.empty()
     try:
         for i in range(device.device_count()):
             info, _ = device.inventory_snapshot(i)
             if info.uuid == uuid:
-                r = device.link_stats(i).last
+                r = check.stats(i).last
     except GsbError:
-        r = LinkResult()
-    return device.link_text(r, uuid)
-
-
-def copyLine(uuid: str) -> str:
-    """gsb_copy_text of GPU `uuid`'s most recent copy probe; "not run" when there is none."""
-    r = CopyResult()
-    try:
-        for i in range(device.device_count()):
-            info, _ = device.inventory_snapshot(i)
-            if info.uuid == uuid:
-                r = device.copy_stats(i).last
-    except GsbError:
-        r = CopyResult()
-    return device.copy_text(r, uuid)
-
-
-def smLine(uuid: str) -> str:
-    """gsb_sm_text of GPU `uuid`'s most recent SM probe; "not run" when there is none."""
-    r = SmResult()
-    try:
-        for i in range(device.device_count()):
-            info, _ = device.inventory_snapshot(i)
-            if info.uuid == uuid:
-                r = device.sm_stats(i).last
-    except GsbError:
-        r = SmResult()
-    return device.sm_text(r, uuid)
-
-
-def clusterLine(uuid: str) -> str:
-    """gsb_cluster_text of GPU `uuid`'s most recent SM-to-SM probe; "not run" when there is none."""
-    r = ClusterResult()
-    try:
-        for i in range(device.device_count()):
-            info, _ = device.inventory_snapshot(i)
-            if info.uuid == uuid:
-                r = device.cluster_stats(i).last
-    except GsbError:
-        r = ClusterResult()
-    return device.cluster_text(r, uuid)
-
-
-def atomicLine(uuid: str) -> str:
-    """gsb_atomic_text of GPU `uuid`'s most recent L2 atomic probe; "not run" when there is none."""
-    r = AtomicResult()
-    try:
-        for i in range(device.device_count()):
-            info, _ = device.inventory_snapshot(i)
-            if info.uuid == uuid:
-                r = device.atomic_stats(i).last
-    except GsbError:
-        r = AtomicResult()
-    return device.atomic_text(r, uuid)
+        r = check.empty()
+    return check.text(r, uuid)
 
 
 def watchXIDs(stop: threading.Event, devs: List[Device], xids: Callable[[List[Device]], None],
@@ -200,87 +177,36 @@ def watchXIDs(stop: threading.Event, devs: List[Device], xids: Callable[[List[De
     L2 atomic probe `atomic_every` (not in the reference) > 0 runs."""
     lib.gsb_health_set_recovery(recovery_cycles if recovered is not None else 0)
     device.set_option(GSB_OPT_ECC_HEALTH, 1 if ecc else 0)
-    device.set_option(GSB_OPT_LINK_PROBE_EVERY_CYCLES, max(0, link_every))
-    device.set_option(GSB_OPT_COPY_PROBE_EVERY_CYCLES, max(0, copy_every))
-    device.set_option(GSB_OPT_SM_PROBE_EVERY_CYCLES, max(0, sm_every))
-    device.set_option(GSB_OPT_CLUSTER_PROBE_EVERY_CYCLES, max(0, cluster_every))
-    device.set_option(GSB_OPT_ATOMIC_PROBE_EVERY_CYCLES, max(0, atomic_every))
+    every = dict(zip(CHECKS, (link_every, copy_every, sm_every, cluster_every, atomic_every)))
+    for check, n in every.items():
+        device.set_option(check.option, max(0, n))
     device.health_start(probe_period_ms, window_bytes)
     try:
-        links_seen, copies_seen, sms_seen, clusters_seen, atomics_seen = {}, {}, {}, {}, {}
+        seen = {check: {} for check in CHECKS}
         while not stop.is_set():
             e = device.health_wait(5000)  # nvidia.go:126
-            if link_every > 0:  # each GPU's most recent link probe, logged once
+            for check in CHECKS:  # each GPU's most recent probe of every check that is on, logged once
+                if every[check] <= 0:
+                    continue
                 try:
                     for i in range(len({extractRealDeviceID(d.ID) for d in devs})):
-                        st = device.link_stats(i)
-                        if st.probes > links_seen.get(i, 0):
-                            links_seen[i] = st.probes
-                            log.info("%s", device.link_text(st.last, device.inventory_snapshot(i)[0].uuid))
-                except GsbError:
-                    pass
-            if copy_every > 0:  # each GPU's most recent copy probe, logged once
-                try:
-                    for i in range(len({extractRealDeviceID(d.ID) for d in devs})):
-                        st = device.copy_stats(i)
-                        if st.probes > copies_seen.get(i, 0):
-                            copies_seen[i] = st.probes
-                            log.info("%s", device.copy_text(st.last, device.inventory_snapshot(i)[0].uuid))
-                except GsbError:
-                    pass
-            if sm_every > 0:  # each GPU's most recent SM probe, logged once
-                try:
-                    for i in range(len({extractRealDeviceID(d.ID) for d in devs})):
-                        st = device.sm_stats(i)
-                        if st.probes > sms_seen.get(i, 0):
-                            sms_seen[i] = st.probes
-                            log.info("%s", device.sm_text(st.last, device.inventory_snapshot(i)[0].uuid))
-                except GsbError:
-                    pass
-            if cluster_every > 0:  # each GPU's most recent SM-to-SM probe, logged once
-                try:
-                    for i in range(len({extractRealDeviceID(d.ID) for d in devs})):
-                        st = device.cluster_stats(i)
-                        if st.probes > clusters_seen.get(i, 0):
-                            clusters_seen[i] = st.probes
-                            log.info("%s", device.cluster_text(st.last, device.inventory_snapshot(i)[0].uuid))
-                except GsbError:
-                    pass
-            if atomic_every > 0:  # each GPU's most recent L2 atomic probe, logged once
-                try:
-                    for i in range(len({extractRealDeviceID(d.ID) for d in devs})):
-                        st = device.atomic_stats(i)
-                        if st.probes > atomics_seen.get(i, 0):
-                            atomics_seen[i] = st.probes
-                            log.info("%s", device.atomic_text(st.last, device.inventory_snapshot(i)[0].uuid))
+                        st = check.stats(i)
+                        if st.probes > seen[check].get(i, 0):
+                            seen[check][i] = st.probes
+                            log.info("%s", check.text(st.last, device.inventory_snapshot(i)[0].uuid))
                 except GsbError:
                     pass
             if e is None:
                 continue
+            raised = next((c for c in CHECKS if e.etype == c.event and every[c] > 0), None)
             if e.etype == GSB_EVENT_ECC and ecc:  # not in the reference: what the GPU records about its HBM
                 log.warning("ECC health of %s: %s: marking it unhealthy", e.uuid.decode(),
                             ECC_CONDITION_NAMES.get(e.edata, "ECC condition ?"))
                 log.warning("%s", eccStatusLine(e.uuid.decode()))
-            elif e.etype == GSB_EVENT_LINK and link_every > 0:  # not in the reference: the GPU's host link
-                log.warning("PCIe link health of %s: %s: marking it unhealthy", e.uuid.decode(),
-                            LINK_CONDITION_NAMES.get(e.edata, "link condition ?"))
-                log.warning("%s", linkLine(e.uuid.decode()))
-            elif e.etype == GSB_EVENT_COPY and copy_every > 0:  # not in the reference: the GPU's DMA copy engines
-                log.warning("copy-engine health of %s: %s: marking it unhealthy", e.uuid.decode(),
-                            COPY_CONDITION_NAMES.get(e.edata, "copy condition ?"))
-                log.warning("%s", copyLine(e.uuid.decode()))
-            elif e.etype == GSB_EVENT_SM and sm_every > 0:  # not in the reference: what the GPU's SMs compute
-                log.warning("SM compute health of %s: %s: marking it unhealthy", e.uuid.decode(),
-                            SM_CONDITION_NAMES.get(e.edata, "SM condition ?"))
-                log.warning("%s", smLine(e.uuid.decode()))
-            elif e.etype == GSB_EVENT_CLUSTER and cluster_every > 0:  # not in the reference: the SM-to-SM network
-                log.warning("SM-to-SM health of %s: %s: marking it unhealthy", e.uuid.decode(),
-                            CLUSTER_CONDITION_NAMES.get(e.edata, "SM-to-SM condition ?"))
-                log.warning("%s", clusterLine(e.uuid.decode()))
-            elif e.etype == GSB_EVENT_ATOMIC and atomic_every > 0:  # not in the reference: the L2's atomic units
-                log.warning("L2 atomic health of %s: %s: marking it unhealthy", e.uuid.decode(),
-                            ATOMIC_CONDITION_NAMES.get(e.edata, "L2 atomic condition ?"))
-                log.warning("%s", atomicLine(e.uuid.decode()))
+            elif raised is not None:
+                log.warning("%s of %s: %s: marking it unhealthy", raised.label, e.uuid.decode(),
+                            raised.conditions.get(e.edata, raised.what + " condition ?"))
+                log.warning("%s", checkLine(raised, e.uuid.decode()))
             elif e.etype == GSB_EVENT_INVENTORY:  # the low-rate NVML refresh disagrees with what is advertised
                 log.warning("inventory of %s changed under the plugin (%d): marking it unhealthy", e.uuid.decode(), e.edata)
             elif e.etype not in (GSB_EVENT_XID, GSB_EVENT_PROBE):  # nvidia.go:127-129
