@@ -12,6 +12,8 @@ import os
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(_HERE, "libgpushare_b200.so")
+# the L1 and constant-cache check's kernels, a module of their own that LIB_PATH loads
+L1_LIB_PATH = os.path.join(_HERE, "libgpushare_b200_l1.so")
 
 GSB_UUID_BUFFER_SIZE = 80
 GSB_BUSID_BUFFER_SIZE = 32
@@ -92,6 +94,17 @@ GSB_SFU_MUFU_WORDS = GSB_SFU_MUFU_FOLDS * (1 + GSB_SFU_RAW)
 GSB_SFU_CORRUPT, GSB_SFU_BOUND, GSB_SFU_FAILED = 1, 2, 4
 SFU_CONDITION_NAMES = {1: "wrong special-function result", 2: "MUFU result outside its envelope",
                        4: "SFU probe failed"}
+GSB_L1_UNIT_L1_LOAD, GSB_L1_UNIT_L1_STORE, GSB_L1_UNIT_NC, GSB_L1_UNIT_TEX, GSB_L1_UNIT_CONST, GSB_L1_UNIT_PARAM = range(6)
+L1_UNIT_NAMES = ["l1_load", "l1_store", "nc", "tex", "const", "param"]
+GSB_L1_FORM_CA, GSB_L1_FORM_PLAIN, GSB_L1_FORM_EVICT_LAST, GSB_L1_FORM_NC = range(4)
+L1_FORM_NAMES = ["ca", "plain", "evict_last", "nc"]
+GSB_L1_UNITS, GSB_L1_THREADS, GSB_L1_REGION_WORDS, GSB_L1_STEPS, GSB_L1_PASSES_DEFAULT, GSB_L1_PASSES_MAX = \
+    6, 1024, 8192, 8, 8, 64
+GSB_L1_TEX_WIDTH, GSB_L1_TEX_ROWS, GSB_L1_TEX_2D_READS, GSB_L1_CONST_WORDS, GSB_L1_PARAM_WORDS = 64, 128, 16384, 4096, 2000
+GSB_L1_RECORDS, GSB_L1_MAX_LAUNCHES, GSB_L1_FORMS = 64, 3, 4
+GSB_L1_ZERO_TEXEL = (1 << 63) - 1
+GSB_L1_CORRUPT, GSB_L1_FAILED = 1, 2
+L1_CONDITION_NAMES = {1: "wrong word through L1, texture or constant cache", 2: "L1 probe failed"}
 GSB_STRESS_UNITS, GSB_STRESS_SETS_MAX, GSB_STRESS_FOLD_THREADS = 4, 4, 128
 GSB_STRESS_DURATION_MAX_MS, GSB_STRESS_SLICE_MAX_MS, GSB_STRESS_SLICE_DEFAULT_MS, GSB_STRESS_SAMPLE_MS = 600000, 100, 50, 25
 GSB_STRESS_UNIT_MASK = 0xF0
@@ -105,8 +118,8 @@ GSB_VARIANT_AUTO, GSB_VARIANT_DIRECT, GSB_VARIANT_CPASYNC, GSB_VARIANT_BULK, GSB
 VARIANT_NAMES = {0: "auto", 1: "direct", 2: "cpasync", 3: "bulk", 4: "bulkw", 5: "bulkd"}
 GSB_PROBE_TIMED, GSB_PROBE_SEED_TABLE = 1, 2
 GSB_EVENT_XID, GSB_EVENT_PROBE, GSB_EVENT_INVENTORY, GSB_EVENT_ECC, GSB_EVENT_LINK, GSB_EVENT_COPY, GSB_EVENT_SM, \
-    GSB_EVENT_CLUSTER, GSB_EVENT_ATOMIC, GSB_EVENT_TENSOR, GSB_EVENT_SFU = 8, 0x100, 0x200, 0x400, 0x800, 0x1000, \
-    0x2000, 0x4000, 0x8000, 0x10000, 0x20000
+    GSB_EVENT_CLUSTER, GSB_EVENT_ATOMIC, GSB_EVENT_TENSOR, GSB_EVENT_SFU, GSB_EVENT_L1 = 8, 0x100, 0x200, 0x400, 0x800, \
+    0x1000, 0x2000, 0x4000, 0x8000, 0x10000, 0x20000, 0x40000
 GSB_PROBE_FAULT_MISMATCH, GSB_PROBE_FAULT_LAUNCH, GSB_PROBE_RECOVERED, GSB_PROBE_FAULT_WEDGED = 1, 2, 3, 4
 GSB_INVENTORY_IDENTITY_CHANGED, GSB_INVENTORY_TOTAL_CHANGED = 1, 2
 GSB_ECC_VALID_MODE, GSB_ECC_VALID_VOLATILE, GSB_ECC_VALID_AGGREGATE, GSB_ECC_VALID_DRAM, GSB_ECC_VALID_REMAP, \
@@ -124,8 +137,8 @@ GSB_ALL_DEVICES = 0xFFFFFFFF
 GSB_OPT_INVENTORY_POLICY, GSB_OPT_WAIT_SPIN_US, GSB_OPT_WATCHDOG_MS, GSB_OPT_INVENTORY_REFRESH_MS, \
     GSB_OPT_TRANSIENT_KEEP_FREE_BYTES, GSB_OPT_SWEEP_EVERY_CYCLES, GSB_OPT_ECC_HEALTH, GSB_OPT_LINK_PROBE_EVERY_CYCLES, \
     GSB_OPT_COPY_PROBE_EVERY_CYCLES, GSB_OPT_SM_PROBE_EVERY_CYCLES, GSB_OPT_CLUSTER_PROBE_EVERY_CYCLES, \
-    GSB_OPT_ATOMIC_PROBE_EVERY_CYCLES, GSB_OPT_TENSOR_PROBE_EVERY_CYCLES, GSB_OPT_SFU_PROBE_EVERY_CYCLES = \
-    1, 2, 3, 4, 5, 6, 7, 8, 9, 10, 11, 12, 13, 14
+    GSB_OPT_ATOMIC_PROBE_EVERY_CYCLES, GSB_OPT_TENSOR_PROBE_EVERY_CYCLES, GSB_OPT_SFU_PROBE_EVERY_CYCLES, \
+    GSB_OPT_L1_PROBE_EVERY_CYCLES = 1, 2, 3, 4, 5, 6, 7, 8, 9, 10, 11, 12, 13, 14, 15
 GSB_INVENTORY_SNAPSHOT, GSB_INVENTORY_LIVE = 0, 1
 GSB_ALLOC_MATCHED, GSB_ALLOC_SINGLE_GPU, GSB_ALLOC_ERR_RESPONSE = 1, 2, 3
 UINT64_MAX = (1 << 64) - 1
@@ -157,6 +170,8 @@ SYMBOLS = [
     "gsb_test_tensor_corrupt", "gsb_test_tensor_operands",
     "gsb_sfu_probe", "gsb_sfu_stats_get", "gsb_sfu_expected", "gsb_sfu_model", "gsb_sfu_vote", "gsb_sfu_conditions",
     "gsb_sfu_text", "gsb_test_sfu_corrupt", "gsb_test_sfu_inputs",
+    "gsb_l1_probe", "gsb_l1_stats_get", "gsb_l1_schedule", "gsb_l1_conditions", "gsb_l1_text", "gsb_test_l1_corrupt",
+    "gsb_test_l1_skip",
     "gsb_allocate", "gsb_allocate_err_response", "gsb_patch_assigned_body",
 ]
 
@@ -867,6 +882,73 @@ class SfuStats(C.Structure):
     ]
 
 
+class L1Cfg(C.Structure):
+    _fields_ = [
+        ("seed", C.c_uint32),
+        ("seed_expect", C.c_uint32),
+        ("units", C.c_uint32),
+        ("passes", C.c_uint32),
+    ]
+
+
+class L1Record(C.Structure):
+    _fields_ = [
+        ("smid", C.c_uint32),
+        ("unit", C.c_uint32),
+        ("form", C.c_uint32),
+        ("reserved0", C.c_uint32),
+        ("offset", C.c_uint64),
+        ("expected", C.c_uint32 * 4),
+        ("observed", C.c_uint32 * 4),
+        ("cls", C.c_uint32),
+        ("alias_bit", C.c_uint32),
+        ("seed_key", C.c_uint32),
+        ("flipped_bits", C.c_uint32),
+    ]
+
+
+class L1UnitResult(C.Structure):
+    _fields_ = [
+        ("status", C.c_int32),
+        ("launches", C.c_uint32),
+        ("sms_covered", C.c_uint32),
+        ("ctas_per_sm", C.c_uint32),
+        ("words_checked", C.c_uint64),
+        ("mismatch_words", C.c_uint64),
+        ("mismatch_bits", C.c_uint64),
+        ("kernel_ns", C.c_uint64),
+    ]
+
+
+class L1Result(C.Structure):
+    _fields_ = [
+        ("status", C.c_int32),
+        ("sm_count", C.c_uint32),
+        ("seed", C.c_uint32),
+        ("seed_expect", C.c_uint32),
+        ("units", C.c_uint32),
+        ("passes", C.c_uint32),
+        ("sms_covered", C.c_uint32),
+        ("n_records", C.c_uint32),
+        ("covered", C.c_uint32 * (GSB_SM_MAX // 32)),
+        ("faulty", C.c_uint32 * (GSB_SM_MAX // 32)),
+        ("unit", L1UnitResult * GSB_L1_UNITS),
+        ("warm_cold", C.c_double * GSB_L1_FORMS),  # by GSB_L1_FORM_*
+        ("records", L1Record * GSB_L1_RECORDS),
+        ("wall_ns", C.c_uint64),
+    ]
+
+
+class L1Stats(C.Structure):
+    _fields_ = [
+        ("probes", C.c_uint64),
+        ("faults", C.c_uint64),
+        ("skipped", C.c_uint64),
+        ("incomplete", C.c_uint64),
+        ("last", L1Result),
+    ]
+
+
 class Pod(C.Structure):
     _fields_ = [
         ("name", C.c_char_p),
@@ -1013,6 +1095,13 @@ def _load() -> C.CDLL:
         "gsb_sfu_model": (C.c_int64, [C.c_uint32, C.c_uint32, u64p, u64p, C.c_size_t, u64p]),
         "gsb_test_sfu_corrupt": (C.c_int, [C.c_uint32, C.c_uint32, C.c_uint32, C.c_uint32, C.c_uint64]),
         "gsb_test_sfu_inputs": (C.c_int, [C.c_uint32, C.c_uint32, C.c_uint32, u64p, u64p, C.c_size_t, u64p, u32p]),
+        "gsb_l1_probe": (C.c_int, [C.c_uint32, C.POINTER(L1Cfg), C.POINTER(L1Result)]),
+        "gsb_l1_stats_get": (C.c_int, [C.c_uint32, C.POINTER(L1Stats)]),
+        "gsb_l1_schedule": (C.c_int64, [C.c_uint32] * 7),
+        "gsb_l1_conditions": (C.c_uint32, [C.POINTER(L1Result)]),
+        "gsb_l1_text": (C.c_int64, [C.POINTER(L1Result), C.c_char_p, C.c_char_p, C.c_size_t]),
+        "gsb_test_l1_corrupt": (C.c_int, [C.c_uint32, C.c_uint32, C.c_uint32, C.c_uint32, C.c_uint64]),
+        "gsb_test_l1_skip": (C.c_int, [C.c_uint32, C.c_uint32]),
         "gsb_allocate": (C.c_int, [C.POINTER(AllocateCtx), C.POINTER(Pod), C.c_uint32, C.c_char_p, C.c_size_t, C.c_void_p, C.c_size_t, C.POINTER(C.c_size_t), C.POINTER(C.c_int32), u32p]),
         "gsb_allocate_err_response": (C.c_int, [C.POINTER(AllocateCtx), C.c_char_p, C.c_size_t, C.c_void_p, C.c_size_t, C.POINTER(C.c_size_t)]),
         "gsb_patch_assigned_body": (C.c_int, [C.c_uint64, C.c_char_p, C.c_size_t]),

@@ -158,6 +158,12 @@ const Check kChecks[] = {
       {GSB_SFU_BOUND, "MUFU result outside its envelope"},
       {GSB_SFU_FAILED, "SFU probe failed"}},
      "SFU condition ?"},
+    {&Flags::probe_l1_every, GSB_OPT_L1_PROBE_EVERY_CYCLES, GSB_EVENT_L1, "L1 and constant-cache health", "l1",
+     [](uint32_t i, const std::string &u) {
+       return probed<gsb_l1_stats>(i, u, gsb_l1_stats_get, gsb_l1_text, nullptr, &gsb_l1_stats::incomplete);
+     },
+     {{GSB_L1_CORRUPT, "wrong word through L1, texture or constant cache"}, {GSB_L1_FAILED, "L1 probe failed"}},
+     "L1 condition ?"},
 };
 constexpr size_t kNumChecks = sizeof kChecks / sizeof kChecks[0];
 

@@ -52,6 +52,7 @@
 #include "gsb_sm_kat.h"
 #include "gsb_tensor_kat.h"
 #include "gsb_sfu_kat.h"
+#include "gsb_l1.h"
 
 namespace {
 
@@ -270,8 +271,10 @@ struct Device {
     std::vector<uint32_t> operands[GSB_SM_UNITS];
   };
   CheckState<gsb_sm_stats, SmHooks> sm;
-  // buffer a wedged SM-check, SM-stress, SM-to-SM or L2 atomic launch still uses (guarded by mu)
+  // buffer a wedged SM-check, SM-stress, SM-to-SM or L2 atomic launch still uses, and the texture objects over it a
+  // wedged L1 launch may still read (guarded by mu)
   void *sm_kept = nullptr;
+  std::vector<cudaTextureObject_t> sm_kept_tex;
   struct StressCorrupt {
     bool armed = false;
     uint32_t smid = 0, unit = 0, index = 0, xr = 0, slice = 0;
@@ -304,6 +307,16 @@ struct Device {
   CheckState<gsb_tensor_stats, SmHooks> tensor;
   // SM special-function health: gsb_test_sfu_corrupt, by GSB_SFU_UNIT_*
   CheckState<gsb_sfu_stats, std::array<SmCorrupt, GSB_SFU_UNITS>> sfu;
+  // L1 and constant-cache health: gsb_test_l1_corrupt by GSB_L1_UNIT_*, gsb_test_l1_skip
+  struct L1Hooks {
+    std::array<SmCorrupt, GSB_L1_UNITS> corrupt;
+    bool skip_armed = false;
+    uint32_t skip_smid = 0;
+  };
+  CheckState<gsb_l1_stats, L1Hooks> l1;
+  // what the L1 probe's CONST unit copies into its bank and its PARAM unit passes as its parameter: the copy is
+  // asynchronous, so its source lives as long as the device
+  std::vector<uint4> l1_const, l1_param;
 
   // persistent worker (gsb_cycle_all / gsb_probe_all): one host thread per device
   std::thread worker;
@@ -333,7 +346,7 @@ struct Global {
   std::atomic<uint64_t> transient_keep_free{1ull << 30};
   std::atomic<uint64_t> sweep_every{0};
   std::atomic<uint64_t> ecc_health{0};
-  std::atomic<uint64_t> check_every[7] = {};  // GSB_OPT_*_PROBE_EVERY_CYCLES, by the check's place in Checks
+  std::atomic<uint64_t> check_every[8] = {};  // GSB_OPT_*_PROBE_EVERY_CYCLES, by the check's place in Checks
 
   // one link or copy probe's pinned buffers at a time in the whole process (the DaemonSet's memory limit covers 8 GPUs)
   std::mutex link_mu;
@@ -533,6 +546,7 @@ int ensure_ready(Device *d) {
   if (pe == cudaSuccess) pe = (cudaError_t)gsb_tensor_kernel_preload(smem_optin);
   if (pe == cudaSuccess) pe = (cudaError_t)gsb_tensor_operands_preload(smem_optin);
   if (pe == cudaSuccess) pe = (cudaError_t)gsb_sfu_kernel_preload(smem_optin);
+  if (pe == cudaSuccess) pe = (cudaError_t)gsb_l1_kernel_preload();
   if (pe == cudaSuccess) pe = (cudaError_t)gsb_sfu_operands_preload(smem_optin);
   if (pe != cudaSuccess) {
     set_error("loading the probe kernels on %s: %s", d->uuid, cudaGetErrorString(pe));
@@ -2079,6 +2093,8 @@ int sm_drain_kept_locked(Device *d) {
   if (!d->wedged && !d->sm_kept) return GSB_OK;
   const int rc = wedged_drain_locked(d);
   if (rc) return rc;
+  for (cudaTextureObject_t t : d->sm_kept_tex) cudaDestroyTextureObject(t);  // before the memory they describe
+  d->sm_kept_tex.clear();
   if (d->sm_kept) cudaFree(d->sm_kept);
   d->sm_kept = nullptr;
   return GSB_OK;
@@ -2103,21 +2119,29 @@ int sm_alloc_locked(Device *d, const char *what, size_t bytes, void **buf) {
   return GSB_OK;
 }
 
-// Owns the transient buffer of one SM-side run whose status is `rc`. On release (at the latest when the run returns)
-// the buffer is freed, unless the run ended in GSB_ERR_TIMEOUT: then a launch still on the stream uses it, and it goes
-// to sm_kept, which sm_drain_kept_locked frees once the stream has drained.
+// Owns the transient buffer of one SM-side run whose status is `rc`, and the texture objects created over it (`tex`).
+// On release (at the latest when the run returns) the objects are destroyed and then the buffer freed, unless the run
+// ended in GSB_ERR_TIMEOUT: then a launch still on the stream uses them, and they go to sm_kept and sm_kept_tex, which
+// sm_drain_kept_locked gives back once the stream has drained.
 struct SmBuffer {
   Device *d;
   const int &rc;
   void *p = nullptr;
+  std::vector<cudaTextureObject_t> tex;
   SmBuffer(Device *d, const int &rc) : d(d), rc(rc) {}
   SmBuffer(const SmBuffer &) = delete;
   ~SmBuffer() { release(); }
   int alloc(const char *what, size_t bytes) { return sm_alloc_locked(d, what, bytes, &p); }
   void release() {
     if (!p) return;
-    if (rc == GSB_ERR_TIMEOUT) d->sm_kept = p;
-    else cudaFree(p);
+    if (rc == GSB_ERR_TIMEOUT) {
+      d->sm_kept = p;
+      d->sm_kept_tex = std::move(tex);
+    } else {
+      for (cudaTextureObject_t t : tex) cudaDestroyTextureObject(t);
+      cudaFree(p);
+    }
+    tex.clear();
     p = nullptr;
   }
 };
@@ -3085,6 +3109,193 @@ int sfu_inputs_locked(Device *d, uint32_t unit, uint32_t op, const uint64_t *a, 
   return rc;
 }
 
+// ------------------------------------------------------------------ L1 and constant-cache health
+
+constexpr uint32_t kL1AllUnits = (1u << GSB_L1_UNITS) - 1;
+constexpr size_t kL1RegionBytes = (size_t)GSB_L1_REGION_WORDS * 16;
+
+// The TEX unit's texture objects over the L1 probe's regions (`rows` rows of GSB_L1_TEX_WIDTH words at buf), added to
+// buf.tex as they are made: one linear resource, then the pitch-2D resource with clamp and with border addressing.
+int l1_textures_locked(Device *d, SmBuffer *buf, uint32_t rows, gsb_l1_args *a) {
+  unsigned long long *const slot[3] = {&a->tex_linear, &a->tex_clamp, &a->tex_border};
+  for (int i = 0; i < 3; i++) {
+    cudaResourceDesc res;
+    memset(&res, 0, sizeof res);
+    if (i == 0) {
+      res.resType = cudaResourceTypeLinear;
+      res.res.linear.devPtr = buf->p;
+      res.res.linear.desc = cudaCreateChannelDesc<uint4>();
+      res.res.linear.sizeInBytes = (size_t)rows * GSB_L1_TEX_WIDTH * 16;
+    } else {
+      res.resType = cudaResourceTypePitch2D;
+      res.res.pitch2D.devPtr = buf->p;
+      res.res.pitch2D.desc = cudaCreateChannelDesc<uint4>();
+      res.res.pitch2D.width = GSB_L1_TEX_WIDTH;
+      res.res.pitch2D.height = rows;
+      res.res.pitch2D.pitchInBytes = GSB_L1_TEX_WIDTH * 16;
+    }
+    cudaTextureDesc td;
+    memset(&td, 0, sizeof td);
+    td.addressMode[0] = td.addressMode[1] = i == 2 ? cudaAddressModeBorder : cudaAddressModeClamp;
+    td.filterMode = cudaFilterModePoint;
+    td.readMode = cudaReadModeElementType;
+    td.normalizedCoords = 0;
+    cudaTextureObject_t t = 0;
+    const cudaError_t e = cudaCreateTextureObject(&t, &res, &td, nullptr);
+    if (e != cudaSuccess) {
+      set_error("creating the L1 probe's texture objects on %s: %s", d->uuid, cudaGetErrorString(e));
+      return GSB_ERR_DRIVER;
+    }
+    buf->tex.push_back(t);
+    *slot[i] = t;
+  }
+  return GSB_OK;
+}
+
+// The median over CTAs of (warm span / (passes - 1)) / cold span of one load form, from spans[cta][form][2].
+double l1_warm_cold(const std::vector<unsigned long long> &spans, uint32_t ctas, uint32_t form, uint32_t passes) {
+  std::vector<double> r;
+  for (uint32_t c = 0; c < ctas && passes > 1; c++) {
+    const unsigned long long cold = spans[((size_t)c * GSB_L1_FORMS + form) * 2];
+    const unsigned long long warm = spans[((size_t)c * GSB_L1_FORMS + form) * 2 + 1];
+    if (cold) r.push_back((double)warm / (passes - 1) / (double)cold);
+  }
+  if (r.empty()) return 0.0;
+  std::sort(r.begin(), r.end());
+  return r.size() % 2 ? r[r.size() / 2] : (r[r.size() / 2 - 1] + r[r.size() / 2]) / 2;
+}
+
+int l1_probe_locked(Device *d, const gsb_l1_cfg *cfg, gsb_l1_result *out) {
+  const uint64_t t0 = now_ns();
+  if (cfg->units & ~kL1AllUnits || cfg->passes > GSB_L1_PASSES_MAX) {
+    set_error("invalid L1 probe configuration (units 0x%x, passes %u)", cfg->units, cfg->passes);
+    return out->status = GSB_ERR_INVALID_ARGUMENT;
+  }
+  out->units = cfg->units ? cfg->units : kL1AllUnits;
+  out->passes = cfg->passes ? cfg->passes : GSB_L1_PASSES_DEFAULT;
+  out->sm_count = d->sm_count;
+  int rc = ensure_ready(d);
+  if (!rc) rc = sm_drain_kept_locked(d);
+  if (rc) return out->status = rc;
+  out->seed = seed_or_fresh(cfg->seed, 0x4C310000u, &d->l1.seed);
+  out->seed_expect = cfg->seed_expect ? cfg->seed_expect : out->seed;
+  const Device::L1Hooks hooks = take_hooks(d, &d->l1.hooks);
+  const uint32_t ctas = d->sm_count, rows = ctas * GSB_L1_TEX_ROWS;
+  const uint64_t words = (uint64_t)ctas * GSB_L1_REGION_WORDS;
+  // one transient buffer: the regions (first, so the texture resources start aligned), the launch log, the spans
+  const size_t log_off = ctas * kL1RegionBytes, span_off = log_off + (sizeof(gsb_l1_log) + 255) / 256 * 256;
+  const size_t span_bytes = (size_t)ctas * GSB_L1_FORMS * 2 * sizeof(unsigned long long);
+  SmBuffer buf(d, rc);
+  rc = buf.alloc("L1 probe", span_off + span_bytes);
+  char *const base = static_cast<char *>(buf.p);
+  gsb_l1_args a;
+  memset(&a, 0, sizeof a);
+  a.log = reinterpret_cast<gsb_l1_log *>(base + log_off);
+  a.buf = reinterpret_cast<uint4 *>(base);
+  a.spans = reinterpret_cast<unsigned long long *>(base + span_off);
+  a.seed = out->seed;
+  a.seed_expect = out->seed_expect;
+  a.passes = out->passes;
+  a.rows = rows;
+  if (rc == GSB_OK && (out->units >> GSB_L1_UNIT_TEX & 1u)) rc = l1_textures_locked(d, &buf, rows, &a);
+  gsb_launch_geom fill_geom;
+  if (rc == GSB_OK) rc = copy_geom_locked(d, GSB_OP_FILL, &fill_geom);
+  // the bank's and the parameter's pattern words
+  const uint32_t key = gsb_seed_key(out->seed);
+  d->l1_const.resize(GSB_L1_CONST_WORDS);
+  d->l1_param.resize(GSB_L1_PARAM_WORDS);
+  for (uint32_t w = 0; w < GSB_L1_CONST_WORDS; w++) {
+    uint32_t l[4];
+    gsb_pattern_word(w, key, l);
+    d->l1_const[w] = make_uint4(l[0], l[1], l[2], l[3]);
+    if (w < GSB_L1_PARAM_WORDS) d->l1_param[w] = d->l1_const[w];
+  }
+  std::vector<unsigned long long> spans(span_bytes / sizeof(unsigned long long));
+  bool first = true;
+  for (uint32_t u = 0; u < GSB_L1_UNITS && rc == GSB_OK; u++) {
+    if (!(out->units >> u & 1u)) continue;
+    gsb_l1_unit_result &ur = out->unit[u];
+    int per_sm = 0;
+    if (gsb_l1_occupancy(u, &per_sm) == cudaSuccess) ur.ctas_per_sm = (uint32_t)per_sm;
+    uint32_t covered[GSB_SM_MAX / 32] = {0};
+    while (ur.launches < GSB_L1_MAX_LAUNCHES && popcount_bitmap(covered) < d->sm_count) {
+      const bool hook = ur.launches == 0;  // test hooks: the unit's first launch only
+      a.hook_smid = hook && hooks.corrupt[u].armed ? hooks.corrupt[u].smid : GSB_SM_MAX;
+      a.hook_index = hooks.corrupt[u].index;
+      a.hook_xr = hooks.corrupt[u].xr;
+      a.skip_smid = hook && u == GSB_L1_UNIT_L1_STORE && hooks.skip_armed ? hooks.skip_smid : GSB_SM_MAX;
+      ur.launches++;
+      int lrc = GSB_OK;
+      if (u <= GSB_L1_UNIT_TEX) {  // the regions hold generation 1 before every launch that reads them
+        gsb_kernel_args fa;
+        memset(&fa, 0, sizeof fa);
+        fa.base = a.buf;
+        fa.n_words = words;
+        fa.seed_write = out->seed;
+        fa.tile_counter = d->tile_counter;
+        gsb_probe_result pr;
+        lrc = copy_launch_locked(d, GSB_OP_FILL, fill_geom, fa, words * 16, words, words * 16 / 10, &pr);
+      } else if (u == GSB_L1_UNIT_CONST) {
+        const cudaError_t e = (cudaError_t)gsb_l1_const_upload(d->l1_const.data(), d->stream);
+        if (e != cudaSuccess) {
+          set_error("copying the L1 probe's constant bank to %s: %s", d->uuid, cudaGetErrorString(e));
+          lrc = GSB_ERR_DRIVER;
+        }
+      }
+      gsb_l1_log log;
+      if (lrc == GSB_OK)
+        lrc = sm_launch_locked(
+            d, "L1 check",
+            [&] { return gsb_l1_kernel_launch(u, ctas, &a, d->l1_param.data(), d->stream); }, a.log, &log,
+            sizeof log, 0, nullptr, &ur.kernel_ns);
+      if (lrc != GSB_OK) {
+        ur.status = rc = lrc;
+        break;
+      }
+      fold_log(log, &ur, out, covered);
+      if (u != GSB_L1_UNIT_L1_LOAD && u != GSB_L1_UNIT_NC) continue;
+      cudaError_t e = cudaMemcpyAsync(spans.data(), a.spans, span_bytes, cudaMemcpyDeviceToHost, d->stream);
+      if (e == cudaSuccess) e = cudaStreamSynchronize(d->stream);
+      if (e != cudaSuccess) {
+        set_error("reading the L1 probe's pass times from %s: %s", d->uuid, cudaGetErrorString(e));
+        ur.status = rc = GSB_ERR_DRIVER;
+        break;
+      }
+      for (uint32_t f = 0; f < GSB_L1_FORMS; f++)
+        if ((u == GSB_L1_UNIT_NC) == (f == GSB_L1_FORM_NC))
+          out->warm_cold[f] = l1_warm_cold(spans, ctas, f, out->passes);
+    }
+    ur.sms_covered = popcount_bitmap(covered);
+    for (int i = 0; i < GSB_SM_MAX / 32; i++) out->covered[i] = first ? covered[i] : out->covered[i] & covered[i];
+    first = false;
+  }
+  out->sms_covered = popcount_bitmap(out->covered);
+  buf.release();
+  // every record classified as an HBM fault record of the same word would be
+  for (uint32_t i = 0; i < out->n_records; i++) {
+    gsb_l1_record &r = out->records[i];
+    gsb_fault_record f;
+    memset(&f, 0, sizeof f);
+    f.offset = r.offset;
+    memcpy(f.expected, r.expected, sizeof f.expected);
+    memcpy(f.observed, r.observed, sizeof f.observed);
+    gsb_fault_classify(&f);
+    r.cls = f.cls;
+    r.alias_bit = f.alias_bit;
+    r.seed_key = f.seed_key;
+    r.flipped_bits = f.flipped_bits;
+  }
+  out->wall_ns = now_ns() - t0;
+  out->status = rc;
+  bool ran = false, short_cover = false;
+  for (const gsb_l1_unit_result &ur : out->unit) {
+    ran = ran || ur.launches != 0;
+    short_cover = short_cover || (ur.launches != 0 && ur.status == GSB_OK && ur.sms_covered < out->sm_count);
+  }
+  count_probe(d, &d->l1.stats, *out, ran, gsb_l1_conditions(out), short_cover ? &d->l1.stats.incomplete : nullptr);
+  return rc;
+}
+
 // ------------------------------------------------------------------ the periodic checks, described once
 
 template <typename Run>
@@ -3117,8 +3328,9 @@ using AtomicCheck = Check<GSB_OPT_ATOMIC_PROBE_EVERY_CYCLES, GSB_EVENT_ATOMIC, &
 using TensorCheck = Check<GSB_OPT_TENSOR_PROBE_EVERY_CYCLES, GSB_EVENT_TENSOR, &Device::tensor, &tensor_probe_locked,
                           &gsb_tensor_conditions>;
 using SfuCheck = Check<GSB_OPT_SFU_PROBE_EVERY_CYCLES, GSB_EVENT_SFU, &Device::sfu, &sfu_probe_locked, &gsb_sfu_conditions>;
+using L1Check = Check<GSB_OPT_L1_PROBE_EVERY_CYCLES, GSB_EVENT_L1, &Device::l1, &l1_probe_locked, &gsb_l1_conditions>;
 // in the order the prober runs them when several are due after the same cycle; G.check_every follows it
-using Checks = std::tuple<LinkCheck, CopyCheck, SmCheck, ClusterCheck, AtomicCheck, TensorCheck, SfuCheck>;
+using Checks = std::tuple<LinkCheck, CopyCheck, SmCheck, ClusterCheck, AtomicCheck, TensorCheck, SfuCheck, L1Check>;
 static_assert(std::tuple_size<Checks>::value == std::extent<decltype(G.check_every)>::value, "one cadence per check");
 
 // f(check, its place in Checks) for every periodic check, in order
@@ -3986,6 +4198,39 @@ int gsb_test_sfu_corrupt(uint32_t idx, uint32_t smid, uint32_t unit, uint32_t in
   c.smid = smid;
   c.index = index;
   c.xr = xr;
+  return GSB_OK;
+}
+
+int gsb_l1_probe(uint32_t idx, const gsb_l1_cfg *cfg, gsb_l1_result *out) {
+  return probe_entry(idx, cfg, out, &L1Check::run);
+}
+
+int gsb_l1_stats_get(uint32_t idx, gsb_l1_stats *out) {
+  return stats_entry(idx, out, [](Device *d) { return &d->l1.stats; });
+}
+
+int gsb_test_l1_corrupt(uint32_t idx, uint32_t smid, uint32_t unit, uint32_t index, uint64_t xr) {
+  std::shared_lock<std::shared_mutex> api_lk(G.api_mu);
+  if (unit >= GSB_L1_UNITS || smid >= GSB_SM_MAX || index >= gsb_l1_hook_words(unit)) return GSB_ERR_INVALID_ARGUMENT;
+  Device *d = device_at(idx);
+  if (!d) return G.inited ? GSB_ERR_NO_DEVICE : GSB_ERR_NOT_INITIALIZED;
+  std::lock_guard<std::mutex> lk(d->smu);
+  Device::SmCorrupt &c = d->l1.hooks.corrupt[unit];
+  c.armed = true;
+  c.smid = smid;
+  c.index = index;
+  c.xr = xr;
+  return GSB_OK;
+}
+
+int gsb_test_l1_skip(uint32_t idx, uint32_t smid) {
+  std::shared_lock<std::shared_mutex> api_lk(G.api_mu);
+  if (smid >= GSB_SM_MAX) return GSB_ERR_INVALID_ARGUMENT;
+  Device *d = device_at(idx);
+  if (!d) return G.inited ? GSB_ERR_NO_DEVICE : GSB_ERR_NOT_INITIALIZED;
+  std::lock_guard<std::mutex> lk(d->smu);
+  d->l1.hooks.skip_armed = true;
+  d->l1.hooks.skip_smid = smid;
   return GSB_OK;
 }
 

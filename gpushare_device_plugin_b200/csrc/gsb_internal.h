@@ -202,6 +202,48 @@ int gsb_sfu_operands_launch(uint32_t unit, uint32_t grid, const gsb_sfu_table_ar
 /* The same preload for the twins. */
 int gsb_sfu_operands_preload(int smem_bytes);
 
+/* What one L1 check launch (l1_check_sm90a.cu) leaves in device memory; the host zeroes it before every launch. Its
+ * leading fields are the SM check's, so fold_log serves it; the host classifies the records afterwards. */
+struct gsb_l1_log {
+  unsigned int covered[GSB_SM_MAX / 32]; /* bit %smid: a CTA of the launch ran there */
+  unsigned int faulty[GSB_SM_MAX / 32];  /* bit %smid: a wrong word there */
+  unsigned long long words;              /* 16-byte words compared */
+  unsigned long long mismatch_words;
+  unsigned long long mismatch_bits;
+  unsigned int count;                    /* records claimed (may pass GSB_L1_RECORDS) */
+  unsigned int pad;
+  gsb_l1_record rec[GSB_L1_RECORDS];
+};
+
+struct gsb_l1_args {
+  gsb_l1_log *log;
+  uint4 *buf;                      /* sm_count regions of GSB_L1_REGION_WORDS words, filled with seed's pattern */
+  unsigned long long *spans;       /* [blockIdx][GSB_L1_FORMS][2]: clock64 span of the cold pass, of the warm passes */
+  unsigned long long tex_linear;   /* TEX: cudaTextureObject_t of buf as one linear uint4 resource */
+  unsigned long long tex_clamp;    /* TEX: buf as a pitch-2D array of GSB_L1_TEX_WIDTH x rows uint4, clamp addressing */
+  unsigned long long tex_border;   /* the same with border addressing */
+  unsigned long long hook_xr;      /* test hook: XORed into lanes 0-1 of observed word hook_index on SM hook_smid */
+  uint32_t seed;                   /* the pattern the buffer, bank and parameters hold; L1_STORE stores generation 2 */
+  uint32_t seed_expect;            /* the pattern the kernels compare against */
+  uint32_t passes;                 /* L1_LOAD and NC */
+  uint32_t rows;                   /* TEX: rows of the 2-D array (GSB_L1_TEX_ROWS per CTA) */
+  uint32_t hook_smid;              /* GSB_SM_MAX: no corrupt hook */
+  uint32_t hook_index;
+  uint32_t skip_smid;              /* L1_STORE: the CTA on this SM stores nothing; GSB_SM_MAX: none */
+  uint32_t reserved0;
+};
+
+/* Enqueue one L1 check launch of GSB_L1_UNIT_* `unit` with `grid` CTAs on `stream`. PARAM launches with `param`
+ * (GSB_L1_PARAM_WORDS words) as its parameter. Returns cudaError_t as int. */
+int gsb_l1_kernel_launch(uint32_t unit, uint32_t grid, const gsb_l1_args *a, const uint4 *param, cudaStream_t stream);
+/* Enqueue the copy of GSB_L1_CONST_WORDS words at `host` into the CONST unit's bank on `stream`; `host` must stay
+ * valid until the copy has run. Returns cudaError_t as int. */
+int gsb_l1_const_upload(const uint4 *host, cudaStream_t stream);
+/* cudaOccupancyMaxActiveBlocksPerMultiprocessor of `unit`'s kernel. Returns cudaError_t as int. */
+int gsb_l1_occupancy(uint32_t unit, int *ctas);
+/* Load the L1 check's kernels into the CURRENT context and ask for the largest L1 (carveout 0) for its buffer units. */
+int gsb_l1_kernel_preload(void);
+
 /* What one SM-stress slice (sm_stress_sm90a.cu) leaves in device memory; the host zeroes it before every slice. */
 struct gsb_stress_log {
   unsigned int covered[GSB_SM_MAX / 32];

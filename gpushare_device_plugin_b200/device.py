@@ -900,6 +900,63 @@ def test_sfu_inputs(idx: int, unit: int, op: int, a, b=None):
 test_sfu_inputs.__test__ = False
 
 
+def l1_probe(idx: int, *, seed: int = 0, seed_expect: int = 0, units: int = 0, passes: int = 0,
+             raise_on_error: bool = True) -> "_abi.L1Result":
+    """L1 and constant-cache probe of device `idx`: each unit (`units`: a mask of 1 << GSB_L1_UNIT_*, 0 = all) on
+    every SM, every word compared on the SM with the pattern for `seed_expect` (0 = `seed`; `seed` 0 = fresh);
+    `passes` per L1_LOAD and NC form (0 = 8). Mismatches are a result, not an error; with raise_on_error=False a failed
+    launch is too (``status`` < 0)."""
+    cfg = _abi.L1Cfg(seed, seed_expect, units, passes)
+    r = _abi.L1Result()
+    rc = lib.gsb_l1_probe(idx, C.byref(cfg), C.byref(r))
+    if raise_on_error:
+        check(rc, f"gsb_l1_probe({idx})")
+    return r
+
+
+def l1_stats(idx: int) -> "_abi.L1Stats":
+    """L1 probes of device `idx` since health_start: count, faults, skipped, incomplete, the last result."""
+    st = _abi.L1Stats()
+    check(lib.gsb_l1_stats_get(idx, C.byref(st)), f"gsb_l1_stats_get({idx})")
+    return st
+
+
+def l1_schedule(unit: int, form: int, pass_: int, cta: int, ctas: int, thread: int, step: int) -> int:
+    """gsb_l1_schedule: the word that read of the L1 probe returns (GSB_L1_ZERO_TEXEL: a border texel), or a negative
+    status for a read the unit does not make."""
+    return int(lib.gsb_l1_schedule(unit, form, pass_, cta, ctas, thread, step))
+
+
+def l1_conditions(r: "_abi.L1Result") -> int:
+    """GSB_L1_* bits an L1 probe result raises."""
+    return lib.gsb_l1_conditions(C.byref(r))
+
+
+def l1_text(r: "_abi.L1Result", uuid: str) -> str:
+    """The one log line both daemons print for an L1 probe result."""
+    need = lib.gsb_l1_text(C.byref(r), uuid.encode(), None, 0)
+    check(int(need), "gsb_l1_text(size)")
+    buf = C.create_string_buffer(int(need))
+    n = lib.gsb_l1_text(C.byref(r), uuid.encode(), buf, int(need))
+    check(int(n), "gsb_l1_text")
+    return buf.raw[: int(n)].decode()
+
+
+def test_l1_corrupt(idx: int, smid: int, unit: int, index: int, xr: int) -> None:
+    """Test hook: on the next L1 probe of `idx`, the CTA on SM `smid` XORs `xr` into lanes 0-1 of its observed word
+    `index` of `unit` just before the compare, in the unit's first launch; once."""
+    check(lib.gsb_test_l1_corrupt(idx, smid, unit, index, xr), f"gsb_test_l1_corrupt({idx})")
+
+
+def test_l1_skip(idx: int, smid: int) -> None:
+    """Test hook: in the next L1 probe of `idx`, the first L1_STORE launch's CTA on SM `smid` stores nothing."""
+    check(lib.gsb_test_l1_skip(idx, smid), f"gsb_test_l1_skip({idx})")
+
+
+test_l1_corrupt.__test__ = False
+test_l1_skip.__test__ = False
+
+
 def fault_classify(offset: int, expected, observed) -> FaultRecord:
     """gsb_fault_classify of one word: cls, alias_bit, seed_key and flipped_bits filled in."""
     rec = FaultRecord(offset, (C.c_uint32 * 4)(*expected), (C.c_uint32 * 4)(*observed))

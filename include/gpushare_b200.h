@@ -45,7 +45,8 @@ extern "C" {
                               gsb_cluster_probe; L2 atomic health (gsb_atomic_*, GSB_EVENT_ATOMIC) likewise, found
                               by gsb_atomic_probe; tensor-core format health (gsb_tensor_*, GSB_EVENT_TENSOR)
                               likewise, found by gsb_tensor_probe; SM special-function health (gsb_sfu_*,
-                              GSB_EVENT_SFU) likewise, found by gsb_sfu_probe */
+                              GSB_EVENT_SFU) likewise, found by gsb_sfu_probe; L1 and constant-cache health
+                              (gsb_l1_*, GSB_EVENT_L1) likewise, found by gsb_l1_probe */
 
 /* = NVML_DEVICE_UUID_BUFFER_SIZE (vendor/.../nvml/nvml.h:1567), used by bindings.go:20 szUUID */
 #define GSB_UUID_BUFFER_SIZE 80
@@ -160,9 +161,14 @@ enum {
                                             a health session and after every Nth cycle, outside gsb_cycle (after the
                                             link, copy, SM, SM-to-SM and L2 atomic probes when they are due), and
                                             raises GSB_EVENT_TENSOR; 0 = off (default): no buffer, no launch */
-  GSB_OPT_SFU_PROBE_EVERY_CYCLES = 14     /* N > 0: each prober thread runs gsb_sfu_probe after its first cycle of a
+  GSB_OPT_SFU_PROBE_EVERY_CYCLES = 14,    /* N > 0: each prober thread runs gsb_sfu_probe after its first cycle of a
+                                            health session and after every Nth cycle, outside gsb_cycle (after the
+                                            link, copy, SM, SM-to-SM, L2 atomic and tensor-core format probes when
+                                            they are due), and raises GSB_EVENT_SFU; 0 = off (default): no buffer, no
+                                            launch */
+  GSB_OPT_L1_PROBE_EVERY_CYCLES = 15      /* N > 0: each prober thread runs gsb_l1_probe after its first cycle of a
                                             health session and after every Nth cycle, outside gsb_cycle (after every
-                                            other periodic probe that is due), and raises GSB_EVENT_SFU; 0 = off
+                                            other periodic probe that is due), and raises GSB_EVENT_L1; 0 = off
                                             (default): no buffer, no launch */
 };
 enum {
@@ -326,8 +332,10 @@ enum {
   GSB_EVENT_ATOMIC = 0x8000,   /* GSB_OPT_ATOMIC_PROBE_EVERY_CYCLES: an L2 atomic condition; edata = one GSB_ATOMIC_* bit */
   GSB_EVENT_TENSOR = 0x10000,  /* GSB_OPT_TENSOR_PROBE_EVERY_CYCLES: a tensor-core format condition; edata = one
                                   GSB_TENSOR_* bit */
-  GSB_EVENT_SFU = 0x20000      /* GSB_OPT_SFU_PROBE_EVERY_CYCLES: an SM special-function condition; edata = one
+  GSB_EVENT_SFU = 0x20000,     /* GSB_OPT_SFU_PROBE_EVERY_CYCLES: an SM special-function condition; edata = one
                                   GSB_SFU_* bit */
+  GSB_EVENT_L1 = 0x40000       /* GSB_OPT_L1_PROBE_EVERY_CYCLES: an L1 or constant-cache condition; edata = one
+                                  GSB_L1_* bit */
 };
 enum { GSB_PROBE_FAULT_MISMATCH = 1, GSB_PROBE_FAULT_LAUNCH = 2, GSB_PROBE_RECOVERED = 3,
        GSB_PROBE_FAULT_WEDGED = 4 /* the launch outlived the completion watchdog */ };
@@ -1590,6 +1598,146 @@ int gsb_test_sfu_corrupt(uint32_t idx, uint32_t smid, uint32_t unit, uint32_t in
  * sin and cos). */
 int gsb_test_sfu_inputs(uint32_t idx, uint32_t unit, uint32_t op, const uint64_t *a, const uint64_t *b, size_t n,
                         uint64_t *results, uint32_t *covered);
+
+/* ---- L1 and constant-cache health (not in the reference; opt-in: GSB_OPT_L1_PROBE_EVERY_CYCLES) ---------------- */
+
+/*
+ * Bit-exact checks of every SM's L1 data cache, read-only and texture paths, constant bank and kernel parameters. Each
+ * unit is one launch of sm_count CTAs of GSB_L1_THREADS; thread 0 of each CTA sets bit %smid of the launch's coverage
+ * bitmap, and a launch that left an SM uncovered is repeated up to GSB_L1_MAX_LAUNCHES times. Every word a CTA reads is
+ * a 16-byte HBM-probe pattern word (gsb_pattern.h) of its own address: the CTA computes the expected word in registers
+ * and compares on the SM, so a wrong word classifies like an HBM fault (gsb_fault_classify: a missed update is STALE,
+ * another address's line ALIASED). The buffer is sm_count regions of GSB_L1_REGION_WORDS words, CTA c owning region c,
+ * filled by the HBM probe's FILL launch before every launch that reads it.
+ *
+ *   L1_LOAD   each CTA reads its region `passes` times with each of ld.global.ca, ld.global and
+ *             ld.global.L1::evict_last; pass 0 in address order (cold), later passes in the orders of
+ *             gsb_l1_schedule (sequential, reversed, lines 4, 16 and 64 KiB apart back to back)        forms 0..2
+ *   L1_STORE  reads its region through L1 (form 0), then each thread stores generation 2 (seed ~seed) over bytes of
+ *             words another warp owns with st.global.u8/u16/u32/v2/v4, then after bar.sync reads every word back
+ *             through L1 (form 1): the byte merge of the two generations                                forms 0, 1
+ *   NC        the passes of L1_LOAD through ld.global.nc                                                 form 0
+ *   TEX       tex1Dfetch of its region (form 0); tex2D with point filtering and unnormalized coordinates over the
+ *             buffer as one 64-word-wide pitch-2D texture, CTA c holding rows [128 c, 128 c + 128), x in [-32, 96)
+ *             and y past the array's first and last rows, once with clamp addressing (form 1: the edge texel) and
+ *             once with border addressing (form 2: 0 outside)
+ *   CONST     a 64 KiB __constant__ bank holding the pattern, read by every thread with uniform indices (form 0) and
+ *             once per CTA with per-thread indices (form 1)
+ *   PARAM     a 32000-byte __grid_constant__ kernel parameter holding the pattern, read likewise
+ *
+ * Warm/cold ratio: each CTA times (clock64) its cold pass and its warm passes of every L1_LOAD and NC form; the result
+ * reports the median over CTAs of (warm span / (passes - 1)) / cold span. It is logged, never judged.
+ */
+enum {
+  GSB_L1_UNIT_L1_LOAD = 0,
+  GSB_L1_UNIT_L1_STORE = 1,
+  GSB_L1_UNIT_NC = 2,
+  GSB_L1_UNIT_TEX = 3,
+  GSB_L1_UNIT_CONST = 4,
+  GSB_L1_UNIT_PARAM = 5
+};
+#define GSB_L1_UNITS 6
+#define GSB_L1_THREADS 1024
+#define GSB_L1_REGION_WORDS 8192   /* 128 KiB per CTA */
+#define GSB_L1_STEPS 8             /* words per thread per pass: GSB_L1_REGION_WORDS / GSB_L1_THREADS */
+#define GSB_L1_PASSES_DEFAULT 8
+#define GSB_L1_PASSES_MAX 64
+#define GSB_L1_TEX_WIDTH 64        /* words per row of the 2-D texture */
+#define GSB_L1_TEX_ROWS 128        /* rows per CTA */
+#define GSB_L1_TEX_2D_READS 16384  /* per CTA and addressing mode: x in [-32, 96) by 128 rows */
+#define GSB_L1_CONST_WORDS 4096    /* 64 KiB */
+#define GSB_L1_PARAM_WORDS 2000    /* 32000 bytes */
+#define GSB_L1_RECORDS 64
+#define GSB_L1_MAX_LAUNCHES 3
+/* the load forms whose warm/cold ratio a result reports, in the order of gsb_l1_result.warm_cold */
+enum { GSB_L1_FORM_CA = 0, GSB_L1_FORM_PLAIN = 1, GSB_L1_FORM_EVICT_LAST = 2, GSB_L1_FORM_NC = 3 };
+#define GSB_L1_FORMS 4
+/* gsb_l1_schedule's answer for a TEX border read outside the array: the texel reads as 0 */
+#define GSB_L1_ZERO_TEXEL 0x7FFFFFFFFFFFFFFFll
+
+typedef struct gsb_l1_cfg {
+  uint32_t seed;        /* the pattern's seed; 0 = fresh per probe */
+  uint32_t seed_expect; /* seed the kernels compare against; 0 = seed */
+  uint32_t units;       /* mask of 1 << GSB_L1_UNIT_*; 0 = all */
+  uint32_t passes;      /* L1_LOAD and NC passes per form, 1..GSB_L1_PASSES_MAX; 0 = GSB_L1_PASSES_DEFAULT */
+} gsb_l1_cfg;
+
+/* One wrong word. offset: byte offset of the expected word's address (buffer units: from the buffer's start; CONST and
+ * PARAM: from the bank's or the parameter's start); cls .. flipped_bits: gsb_fault_classify's, filled by the host. */
+typedef struct gsb_l1_record {
+  uint32_t smid, unit, form, reserved0;
+  uint64_t offset;
+  uint32_t expected[4];
+  uint32_t observed[4];
+  uint32_t cls, alias_bit, seed_key, flipped_bits;
+} gsb_l1_record;
+
+typedef struct gsb_l1_unit_result {
+  int32_t status;          /* GSB_OK, or the first failed launch's gsb_status (GSB_ERR_TIMEOUT: outlived the watchdog) */
+  uint32_t launches;       /* 0 = the unit did not run */
+  uint32_t sms_covered;    /* distinct %smid over its launches */
+  uint32_t ctas_per_sm;    /* cudaOccupancyMaxActiveBlocksPerMultiprocessor of its kernel (logged only) */
+  uint64_t words_checked;  /* 16-byte words compared, over every CTA of every launch */
+  uint64_t mismatch_words, mismatch_bits;
+  uint64_t kernel_ns;      /* CUDA-event time of its launches */
+} gsb_l1_unit_result;
+
+typedef struct gsb_l1_result {
+  int32_t status;          /* GSB_OK iff every unit asked for ran every launch (mismatches are a result) */
+  uint32_t sm_count;       /* the device's multiProcessorCount = the grid of every launch */
+  uint32_t seed, seed_expect, units, passes;
+  uint32_t sms_covered;    /* SMs covered by every unit that ran */
+  uint32_t n_records;      /* records filled (the first GSB_L1_RECORDS mismatches) */
+  uint32_t covered[GSB_SM_MAX / 32];  /* their bitmap, bit smid */
+  uint32_t faulty[GSB_SM_MAX / 32];   /* SMs with at least one wrong word */
+  gsb_l1_unit_result unit[GSB_L1_UNITS];
+  double warm_cold[GSB_L1_FORMS];     /* by GSB_L1_FORM_*: median warm/cold ratio; 0 = not measured */
+  gsb_l1_record records[GSB_L1_RECORDS];
+  uint64_t wall_ns;        /* host time of the whole call */
+} gsb_l1_result;
+
+/* Conditions (gsb_l1_conditions), from the units that ran only. Coverage short of sm_count after the relaunches is
+ * counted (gsb_l1_stats.incomplete) and logged, never a condition. */
+enum {
+  GSB_L1_CORRUPT = 1u, /* a word read through L1, the read-only path, the texture path, the constant bank or the
+                          kernel parameters differs from its pattern word on some SM */
+  GSB_L1_FAILED = 2u   /* a launch failed or outlived the watchdog */
+};
+
+/* L1 probes of one device since gsb_health_start (counters restart with it; gsb_l1_probe calls count too). */
+typedef struct gsb_l1_stats {
+  uint64_t probes;     /* L1 probes run */
+  uint64_t faults;     /* of which raised at least one GSB_L1_* condition */
+  uint64_t skipped;    /* probes that ran no unit (buffer not allocatable): no condition, no event */
+  uint64_t incomplete; /* probes in which some unit covered fewer than sm_count SMs */
+  gsb_l1_result last;
+} gsb_l1_stats;
+
+/* Holds the device while it runs; each launch under the completion watchdog. One transient buffer of sm_count x
+ * 128 KiB plus the launch log, taken only while GSB_OPT_TRANSIENT_KEEP_FREE_BYTES stays free; a probe that cannot take
+ * it returns GSB_ERR_OUT_OF_MEMORY and counts as skipped. */
+int gsb_l1_probe(uint32_t idx, const gsb_l1_cfg *cfg, gsb_l1_result *out);
+int gsb_l1_stats_get(uint32_t idx, gsb_l1_stats *out);
+/* Pure: the word read number `step` of thread `thread` reads in pass `pass` of form `form` of `unit`, in CTA `cta` of
+ * `ctas`: the buffer word index (TEX: of the texel whose value the read returns; GSB_L1_ZERO_TEXEL for a border read
+ * outside the array), or the bank's or parameter's word index for CONST and PARAM. Negative gsb_status for a tuple
+ * the unit does not read (pass >= GSB_L1_PASSES_MAX, cta >= ctas, step past the form's reads, ...). */
+int64_t gsb_l1_schedule(uint32_t unit, uint32_t form, uint32_t pass, uint32_t cta, uint32_t ctas, uint32_t thread,
+                        uint32_t step);
+/* Pure: GSB_L1_* bits that hold for a result (see above). */
+uint32_t gsb_l1_conditions(const gsb_l1_result *r);
+/* Pure: the one-line text both daemons log for a result. uuid may be NULL. Returns like gsb_sm_text. */
+int64_t gsb_l1_text(const gsb_l1_result *r, const char *uuid, char *buf, size_t cap);
+/* test hook: on the next gsb_l1_probe of device idx, the CTA running on SM `smid` XORs xr into lanes 0-1 of its
+ * observed word `index` of `unit` just before the compare, in the unit's first launch only. index: L1_LOAD and NC the
+ * region word read in pass 0 of form 0, L1_STORE the region word read back, TEX [0, 8192) the 1-D read of that region
+ * word and then the 2-D reads of forms 1 and 2 (GSB_L1_TEX_2D_READS each), CONST and PARAM the word of the per-thread
+ * reads. Refused before any device is touched: unit or smid out of range, or index past the unit's words. */
+int gsb_test_l1_corrupt(uint32_t idx, uint32_t smid, uint32_t unit, uint32_t index, uint64_t xr);
+/* test hook: in the next gsb_l1_probe of device idx, the CTA of the first L1_STORE launch on SM `smid` stores nothing,
+ * so every word it owed reads back as generation 1 (STALE). Refused before any device is touched when smid is out of
+ * range. */
+int gsb_test_l1_skip(uint32_t idx, uint32_t smid);
 
 /* ---- Allocate (a12, a13): wire bytes in, wire bytes out ---------------------------------- */
 

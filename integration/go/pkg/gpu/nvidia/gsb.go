@@ -98,6 +98,7 @@ const (
 	gsbEventAtomic    = uint64(C.GSB_EVENT_ATOMIC)    // opt-in L2 atomic health: Edata = one of the gsbAtomic* conditions below
 	gsbEventTensor    = uint64(C.GSB_EVENT_TENSOR)    // opt-in tensor-core format health: Edata = one of the gsbTensor* conditions below
 	gsbEventSFU       = uint64(C.GSB_EVENT_SFU)       // opt-in SM special-function health: Edata = one of the gsbSFU* conditions below
+	gsbEventL1        = uint64(C.GSB_EVENT_L1)        // opt-in L1 and constant-cache health: Edata = one of the gsbL1* conditions below
 )
 
 const (
@@ -136,6 +137,11 @@ const (
 	gsbSFUCorrupt = uint64(C.GSB_SFU_CORRUPT) // a conversion, divide, warp-collective or MUFU result is wrong on some SM
 	gsbSFUBound   = uint64(C.GSB_SFU_BOUND)   // a MUFU result every SM agrees on lies outside its envelope
 	gsbSFUFailed  = uint64(C.GSB_SFU_FAILED)  // an SFU-check launch failed or outlived the watchdog
+)
+
+const (
+	gsbL1Corrupt = uint64(C.GSB_L1_CORRUPT) // a word read through L1, texture, constant bank or kernel parameters is wrong on some SM
+	gsbL1Failed  = uint64(C.GSB_L1_FAILED)  // an L1-check launch failed or outlived the watchdog
 )
 
 const (
@@ -575,6 +581,34 @@ func gsbSFULine(idx uint, uuid string) string {
 	}
 	buf := make([]byte, int(need))
 	n := C.gsb_sfu_text(&st.last, cu, (*C.char)(unsafe.Pointer(&buf[0])), C.size_t(len(buf)))
+	if n < 0 {
+		return ""
+	}
+	return string(buf[:int(n)])
+}
+
+// gsbEnableL1Health turns on L1 and constant-cache health: each prober runs gsb_l1_probe after its first cycle of a
+// session and after every `every`-th cycle. Call it before gsbHealthStart.
+func gsbEnableL1Health(every uint64) error {
+	return gsbErr(C.gsb_set_option(C.GSB_OPT_L1_PROBE_EVERY_CYCLES, C.uint64_t(every)))
+}
+
+// gsbL1Line is the one log line of GPU idx's most recent L1 and constant-cache probe ("not run" when there is none):
+// what a plugin logs before marking a GPU unhealthy on a GSB_EVENT_L1 event.
+func gsbL1Line(idx uint, uuid string) string {
+	st := (*C.gsb_l1_stats)(C.calloc(1, C.size_t(unsafe.Sizeof(C.gsb_l1_stats{}))))
+	defer C.free(unsafe.Pointer(st))
+	if C.gsb_l1_stats_get(C.uint32_t(idx), st) != C.GSB_OK {
+		*st = C.gsb_l1_stats{}
+	}
+	cu := C.CString(uuid)
+	defer C.free(unsafe.Pointer(cu))
+	need := C.gsb_l1_text(&st.last, cu, nil, 0)
+	if need <= 0 {
+		return ""
+	}
+	buf := make([]byte, int(need))
+	n := C.gsb_l1_text(&st.last, cu, (*C.char)(unsafe.Pointer(&buf[0])), C.size_t(len(buf)))
 	if n < 0 {
 		return ""
 	}
