@@ -21,9 +21,11 @@ $NVCC $FLAGS -Xptxas -v -c $SRC/tensor_operands_sm90a.cu -o build/tensor_operand
 $NVCC $FLAGS -Xptxas -v -c $SRC/sfu_check_sm90a.cu -o build/sfu_check_sm90a.o 2> build/ptxas_sfu_check.log || { cat build/ptxas_sfu_check.log; exit 1; }
 $NVCC $FLAGS -Xptxas -v -c $SRC/sfu_operands_sm90a.cu -o build/sfu_operands_sm90a.o 2> build/ptxas_sfu_operands.log || { cat build/ptxas_sfu_operands.log; exit 1; }
 $NVCC $FLAGS -Xptxas -v -c $SRC/l1_check_sm90a.cu -o build/l1_check_sm90a.o 2> build/ptxas_l1_check.log || { cat build/ptxas_l1_check.log; exit 1; }
+$NVCC $FLAGS -Xptxas -v -c $SRC/l1_table_sm90a.cu -o build/l1_table_sm90a.o 2> build/ptxas_l1_table.log || { cat build/ptxas_l1_table.log; exit 1; }
 # the L1 and constant-cache check's kernels are a module of their own: its 64 KiB __constant__ bank fills the whole user
-# bank of the module that declares it, and the kernels of libgpushare_b200.so keep their recorded SASS
-$NVCC -shared -gencode arch=compute_90a,code=sm_90a -cudart static -o $PKG/libgpushare_b200_l1.so build/l1_check_sm90a.o
+# bank of the module that declares it, and the kernels of libgpushare_b200.so keep their recorded SASS; their test-only
+# twins (l1_table_sm90a.cu, a CUDA module of its own with its own bank) go into the same library
+$NVCC -shared -gencode arch=compute_90a,code=sm_90a -cudart static -o $PKG/libgpushare_b200_l1.so build/l1_check_sm90a.o build/l1_table_sm90a.o
 $NVCC $FLAGS -c $SRC/gsb_device.cu -o build/gsb_device.o
 g++ -O2 -std=c++17 -fPIC -Wall -c $SRC/gsb_wire.cc -o build/gsb_wire.o
 g++ -O2 -std=c++17 -fPIC -Wall -c $SRC/gsb_fault.cc -o build/gsb_fault.o

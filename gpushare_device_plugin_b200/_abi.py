@@ -105,6 +105,9 @@ GSB_L1_RECORDS, GSB_L1_MAX_LAUNCHES, GSB_L1_FORMS = 64, 3, 4
 GSB_L1_ZERO_TEXEL = (1 << 63) - 1
 GSB_L1_CORRUPT, GSB_L1_FAILED = 1, 2
 L1_CONDITION_NAMES = {1: "wrong word through L1, texture or constant cache", 2: "L1 probe failed"}
+# gsb_test_l1_table
+GSB_L1_TABLE_MAX, GSB_L1_TABLE_EXPECTED_MAX, GSB_L1_TABLE_REGION_MAX, GSB_L1_TABLE_ROUNDS_MAX = 1 << 20, 1 << 24, 131072, 8
+GSB_L1_STORE_WORD_BITS, GSB_L1_TABLE_RESIDENT, GSB_L1_TABLE_READ_OWN, GSB_L1_TEX_1D = 17, 1, 2, 0x80000000
 GSB_STRESS_UNITS, GSB_STRESS_SETS_MAX, GSB_STRESS_FOLD_THREADS = 4, 4, 128
 GSB_STRESS_DURATION_MAX_MS, GSB_STRESS_SLICE_MAX_MS, GSB_STRESS_SLICE_DEFAULT_MS, GSB_STRESS_SAMPLE_MS = 600000, 100, 50, 25
 GSB_STRESS_UNIT_MASK = 0xF0
@@ -171,7 +174,7 @@ SYMBOLS = [
     "gsb_sfu_probe", "gsb_sfu_stats_get", "gsb_sfu_expected", "gsb_sfu_model", "gsb_sfu_vote", "gsb_sfu_conditions",
     "gsb_sfu_text", "gsb_test_sfu_corrupt", "gsb_test_sfu_inputs",
     "gsb_l1_probe", "gsb_l1_stats_get", "gsb_l1_schedule", "gsb_l1_conditions", "gsb_l1_text", "gsb_test_l1_corrupt",
-    "gsb_test_l1_skip",
+    "gsb_test_l1_skip", "gsb_test_l1_table",
     "gsb_allocate", "gsb_allocate_err_response", "gsb_patch_assigned_body",
 ]
 
@@ -1102,6 +1105,7 @@ def _load() -> C.CDLL:
         "gsb_l1_text": (C.c_int64, [C.POINTER(L1Result), C.c_char_p, C.c_char_p, C.c_size_t]),
         "gsb_test_l1_corrupt": (C.c_int, [C.c_uint32, C.c_uint32, C.c_uint32, C.c_uint32, C.c_uint64]),
         "gsb_test_l1_skip": (C.c_int, [C.c_uint32, C.c_uint32]),
+        "gsb_test_l1_table": (C.c_int, [C.c_uint32, C.c_uint32, u32p, C.c_size_t, u32p, C.c_size_t, C.c_uint32]),
         "gsb_allocate": (C.c_int, [C.POINTER(AllocateCtx), C.POINTER(Pod), C.c_uint32, C.c_char_p, C.c_size_t, C.c_void_p, C.c_size_t, C.POINTER(C.c_size_t), C.POINTER(C.c_int32), u32p]),
         "gsb_allocate_err_response": (C.c_int, [C.POINTER(AllocateCtx), C.c_char_p, C.c_size_t, C.c_void_p, C.c_size_t, C.POINTER(C.c_size_t)]),
         "gsb_patch_assigned_body": (C.c_int, [C.c_uint64, C.c_char_p, C.c_size_t]),

@@ -314,6 +314,14 @@ struct Device {
     uint32_t skip_smid = 0;
   };
   CheckState<gsb_l1_stats, L1Hooks> l1;
+  // gsb_test_l1_table, by GSB_L1_UNIT_* (guarded by smu): a twin's table and expected words, taken by the next probe
+  // that runs the unit
+  struct L1Table {
+    bool armed = false;
+    uint32_t region_words = 0;
+    std::vector<uint32_t> table, expected;
+  };
+  std::array<L1Table, GSB_L1_UNITS> l1_table;
   // what the L1 probe's CONST unit copies into its bank and its PARAM unit passes as its parameter: the copy is
   // asynchronous, so its source lives as long as the device
   std::vector<uint4> l1_const, l1_param;
@@ -3112,7 +3120,6 @@ int sfu_inputs_locked(Device *d, uint32_t unit, uint32_t op, const uint64_t *a, 
 // ------------------------------------------------------------------ L1 and constant-cache health
 
 constexpr uint32_t kL1AllUnits = (1u << GSB_L1_UNITS) - 1;
-constexpr size_t kL1RegionBytes = (size_t)GSB_L1_REGION_WORDS * 16;
 
 // The TEX unit's texture objects over the L1 probe's regions (`rows` rows of GSB_L1_TEX_WIDTH words at buf), added to
 // buf.tex as they are made: one linear resource, then the pitch-2D resource with clamp and with border addressing.
@@ -3180,13 +3187,28 @@ int l1_probe_locked(Device *d, const gsb_l1_cfg *cfg, gsb_l1_result *out) {
   out->seed = seed_or_fresh(cfg->seed, 0x4C310000u, &d->l1.seed);
   out->seed_expect = cfg->seed_expect ? cfg->seed_expect : out->seed;
   const Device::L1Hooks hooks = take_hooks(d, &d->l1.hooks);
+  // gsb_test_l1_table: taken by the first probe that runs its unit
+  std::array<Device::L1Table, GSB_L1_UNITS> chosen;
+  uint32_t region_max = GSB_L1_REGION_WORDS;
+  size_t table_bytes = 0, expected_bytes = 0;
+  {
+    std::lock_guard<std::mutex> lk(d->smu);
+    for (uint32_t u = 0; u < GSB_L1_UNITS; u++) {
+      if (!(out->units >> u & 1u) || !d->l1_table[u].armed) continue;
+      chosen[u] = std::exchange(d->l1_table[u], Device::L1Table{});
+      region_max = std::max(region_max, chosen[u].region_words);
+      table_bytes = std::max(table_bytes, (4 * chosen[u].table.size() + 255) / 256 * 256);
+      expected_bytes = std::max(expected_bytes, 4 * chosen[u].expected.size());
+    }
+  }
   const uint32_t ctas = d->sm_count, rows = ctas * GSB_L1_TEX_ROWS;
-  const uint64_t words = (uint64_t)ctas * GSB_L1_REGION_WORDS;
-  // one transient buffer: the regions (first, so the texture resources start aligned), the launch log, the spans
-  const size_t log_off = ctas * kL1RegionBytes, span_off = log_off + (sizeof(gsb_l1_log) + 255) / 256 * 256;
+  // one transient buffer: the regions (first, so the texture resources start aligned), the launch log, the spans, a
+  // chosen table and its expected words
+  const size_t log_off = ctas * (size_t)region_max * 16, span_off = log_off + (sizeof(gsb_l1_log) + 255) / 256 * 256;
   const size_t span_bytes = (size_t)ctas * GSB_L1_FORMS * 2 * sizeof(unsigned long long);
+  const size_t table_off = span_off + (span_bytes + 255) / 256 * 256, expected_off = table_off + table_bytes;
   SmBuffer buf(d, rc);
-  rc = buf.alloc("L1 probe", span_off + span_bytes);
+  rc = buf.alloc("L1 probe", expected_off + expected_bytes);
   char *const base = static_cast<char *>(buf.p);
   gsb_l1_args a;
   memset(&a, 0, sizeof a);
@@ -3215,6 +3237,27 @@ int l1_probe_locked(Device *d, const gsb_l1_cfg *cfg, gsb_l1_result *out) {
   for (uint32_t u = 0; u < GSB_L1_UNITS && rc == GSB_OK; u++) {
     if (!(out->units >> u & 1u)) continue;
     gsb_l1_unit_result &ur = out->unit[u];
+    const Device::L1Table &tb = chosen[u];
+    gsb_l1_table_args ta;
+    memset(&ta, 0, sizeof ta);
+    if (tb.armed) {
+      ta.table = reinterpret_cast<const uint32_t *>(base + table_off);
+      ta.expected = reinterpret_cast<const uint32_t *>(base + expected_off);
+      ta.n = (uint32_t)tb.table.size();
+      ta.region_words = tb.region_words;
+      cudaError_t e = cudaMemcpyAsync(base + table_off, tb.table.data(), 4 * tb.table.size(), cudaMemcpyHostToDevice,
+                                      d->stream);
+      if (e == cudaSuccess && !tb.expected.empty())
+        e = cudaMemcpyAsync(base + expected_off, tb.expected.data(), 4 * tb.expected.size(), cudaMemcpyHostToDevice,
+                            d->stream);
+      if (e != cudaSuccess) {
+        set_error("uploading the L1 probe's chosen table to %s: %s", d->uuid, cudaGetErrorString(e));
+        ur.status = rc = GSB_ERR_DRIVER;
+        break;
+      }
+    }
+    // a chosen table of a buffer unit sets the region size
+    const uint64_t words = (uint64_t)ctas * (tb.armed && u < GSB_L1_UNIT_TEX ? tb.region_words : GSB_L1_REGION_WORDS);
     int per_sm = 0;
     if (gsb_l1_occupancy(u, &per_sm) == cudaSuccess) ur.ctas_per_sm = (uint32_t)per_sm;
     uint32_t covered[GSB_SM_MAX / 32] = {0};
@@ -3246,7 +3289,11 @@ int l1_probe_locked(Device *d, const gsb_l1_cfg *cfg, gsb_l1_result *out) {
       if (lrc == GSB_OK)
         lrc = sm_launch_locked(
             d, "L1 check",
-            [&] { return gsb_l1_kernel_launch(u, ctas, &a, d->l1_param.data(), d->stream); }, a.log, &log,
+            [&] {
+              return tb.armed ? gsb_l1_table_launch(u, ctas, &a, &ta, d->l1_const.data(), d->l1_param.data(), d->stream)
+                              : gsb_l1_kernel_launch(u, ctas, &a, d->l1_param.data(), d->stream);
+            },
+            a.log, &log,
             sizeof log, 0, nullptr, &ur.kernel_ns);
       if (lrc != GSB_OK) {
         ur.status = rc = lrc;
@@ -3263,7 +3310,7 @@ int l1_probe_locked(Device *d, const gsb_l1_cfg *cfg, gsb_l1_result *out) {
       }
       for (uint32_t f = 0; f < GSB_L1_FORMS; f++)
         if ((u == GSB_L1_UNIT_NC) == (f == GSB_L1_FORM_NC))
-          out->warm_cold[f] = l1_warm_cold(spans, ctas, f, out->passes);
+          out->warm_cold[f] = l1_warm_cold(spans, ctas, f, tb.armed ? ta.n / ta.region_words : out->passes);
     }
     ur.sms_covered = popcount_bitmap(covered);
     for (int i = 0; i < GSB_SM_MAX / 32; i++) out->covered[i] = first ? covered[i] : out->covered[i] & covered[i];
@@ -4220,6 +4267,27 @@ int gsb_test_l1_corrupt(uint32_t idx, uint32_t smid, uint32_t unit, uint32_t ind
   c.smid = smid;
   c.index = index;
   c.xr = xr;
+  return GSB_OK;
+}
+
+int gsb_test_l1_table(uint32_t idx, uint32_t unit, const uint32_t *table, size_t n, const uint32_t *expected,
+                      size_t n_expected, uint32_t region_words) {
+  std::shared_lock<std::shared_mutex> api_lk(G.api_mu);
+  // refused here, before any device is touched
+  if (unit >= GSB_L1_UNITS || (table && !gsb_l1_table_valid(unit, table, n, expected, n_expected, region_words)))
+    return GSB_ERR_INVALID_ARGUMENT;
+  Device *d = device_at(idx);
+  if (!d) return G.inited ? GSB_ERR_NO_DEVICE : GSB_ERR_NOT_INITIALIZED;
+  Device::L1Table tb;
+  if (table) {
+    if (n_expected != gsb_l1_table_expected_per_cta(unit, n, region_words) * d->sm_count) return GSB_ERR_INVALID_ARGUMENT;
+    tb.armed = true;
+    tb.region_words = region_words;
+    tb.table.assign(table, table + n);
+    if (n_expected) tb.expected.assign(expected, expected + n_expected);
+  }
+  std::lock_guard<std::mutex> lk(d->smu);
+  d->l1_table[unit] = std::move(tb);
   return GSB_OK;
 }
 

@@ -236,6 +236,19 @@ struct gsb_l1_args {
 /* Enqueue one L1 check launch of GSB_L1_UNIT_* `unit` with `grid` CTAs on `stream`. PARAM launches with `param`
  * (GSB_L1_PARAM_WORDS words) as its parameter. Returns cudaError_t as int. */
 int gsb_l1_kernel_launch(uint32_t unit, uint32_t grid, const gsb_l1_args *a, const uint4 *param, cudaStream_t stream);
+/* What a test-only twin l1_from_table<UNIT> reads besides gsb_l1_args (gsb_test_l1_table, include/gpushare_b200.h). */
+struct gsb_l1_table_args {
+  const uint32_t *table;     /* n entries */
+  const uint32_t *expected;  /* L1_STORE: [cta][region word][4]; TEX: [cta][read][2]; else unused */
+  uint32_t n;
+  uint32_t region_words;     /* words of each CTA's region (TEX, CONST, PARAM: the fixed size) */
+};
+
+/* Enqueue one launch of `unit`'s twin (l1_table_sm90a.cu) with `grid` CTAs on `stream`, as gsb_l1_kernel_launch; CONST
+ * first enqueues the copy of GSB_L1_CONST_WORDS words at `bank` into the twin's own bank (`bank` must stay valid until
+ * it has run). Returns cudaError_t as int. */
+int gsb_l1_table_launch(uint32_t unit, uint32_t grid, const gsb_l1_args *a, const gsb_l1_table_args *t,
+                        const uint4 *bank, const uint4 *param, cudaStream_t stream);
 /* Enqueue the copy of GSB_L1_CONST_WORDS words at `host` into the CONST unit's bank on `stream`; `host` must stay
  * valid until the copy has run. Returns cudaError_t as int. */
 int gsb_l1_const_upload(const uint4 *host, cudaStream_t stream);

@@ -3,9 +3,11 @@
  * conditions and the one log line both daemons print. No CUDA, no state.
  */
 #include <stdio.h>
+#include <algorithm>
 #include <string.h>
 
 #include <string>
+#include <vector>
 
 #include "../../include/gpushare_b200.h"
 #include "gsb_l1.h"
@@ -16,6 +18,64 @@ const char *const kUnitName[GSB_L1_UNITS] = {"l1_load", "l1_store", "nc", "tex",
 const char *const kFormName[GSB_L1_FORMS] = {"ca", "plain", "evict_last", "nc"};
 
 }  // namespace
+
+bool gsb_l1_table_valid(uint32_t unit, const uint32_t *table, size_t n, const uint32_t *expected, size_t n_expected,
+                        uint32_t region_words) {
+  if (unit >= GSB_L1_UNITS || !table || n == 0 || n > GSB_L1_TABLE_MAX || n_expected > GSB_L1_TABLE_EXPECTED_MAX)
+    return false;
+  const uint32_t fixed = gsb_l1_table_fixed_words(unit);
+  if (fixed ? region_words != fixed
+            : region_words == 0 || region_words % GSB_L1_THREADS || region_words > GSB_L1_TABLE_REGION_MAX)
+    return false;
+  const uint64_t per_cta = gsb_l1_table_expected_per_cta(unit, n, region_words);
+  if (per_cta == 0 ? n_expected != 0 : !expected || n_expected == 0 || n_expected % per_cta) return false;
+  switch (unit) {
+    case GSB_L1_UNIT_L1_LOAD:
+    case GSB_L1_UNIT_NC:
+      if (n % region_words) return false;
+      break;
+    case GSB_L1_UNIT_L1_STORE: {
+      const size_t rounds = (n - 1) / GSB_L1_THREADS;
+      if (region_words > 1u << GSB_L1_STORE_WORD_BITS || (n - 1) % GSB_L1_THREADS || rounds == 0 ||
+          rounds > GSB_L1_TABLE_ROUNDS_MAX || table[0] & ~(GSB_L1_TABLE_RESIDENT | GSB_L1_TABLE_READ_OWN))
+        return false;
+      std::vector<uint16_t> stored(region_words);  // the bytes of each word stored so far in the round
+      for (size_t r = 0; r < rounds; r++) {
+        std::fill(stored.begin(), stored.end(), 0);
+        for (uint32_t t = 0; t < GSB_L1_THREADS; t++) {
+          const uint32_t e = table[1 + r * GSB_L1_THREADS + t];
+          if (e == 0) continue;
+          const uint32_t code = e >> (GSB_L1_STORE_WORD_BITS + 4) & 7u, w = gsb_l1_entry_word(e);
+          const uint32_t lo = gsb_l1_entry_lo(e), width = gsb_l1_entry_width(e);
+          if (code == 0 || code > 5 || gsb_l1_entry_gen(e) == 0 || w >= region_words || lo % width || lo + width > 16)
+            return false;
+          const uint32_t mask = ((1u << width) - 1u) << lo;
+          if (stored[w] & mask) return false;  // a data race: no reference can say which byte wins
+          stored[w] = (uint16_t)(stored[w] | mask);
+        }
+      }
+      return true;
+    }
+    case GSB_L1_UNIT_TEX:
+      if (n % (2 * GSB_L1_THREADS)) return false;
+      for (size_t r = 0; r < n / 2; r++) {
+        const int32_t x = (int32_t)table[2 * r], y = (int32_t)table[2 * r + 1];
+        const int32_t lim = 1 << 21;  // (float)(band + y) + 0.5f stays exact
+        if (table[2 * r + 1] == GSB_L1_TEX_1D ? x < 0 || x >= (int32_t)GSB_L1_REGION_WORDS
+                                               : x <= -lim || x >= lim || y <= -lim || y >= lim)
+          return false;
+      }
+      for (size_t i = 0; i < n_expected; i++)
+        if ((int32_t)expected[i] < -1) return false;
+      return true;
+    default:  // CONST, PARAM
+      if (n % GSB_L1_THREADS) return false;
+      break;
+  }
+  for (size_t i = 0; i < n; i++)  // word indices inside the region, the bank or the parameter
+    if (table[i] >= region_words) return false;
+  return true;
+}
 
 extern "C" {
 

@@ -7,6 +7,7 @@
 #ifndef GSB_L1_H_
 #define GSB_L1_H_
 
+#include <stddef.h>
 #include <stdint.h>
 
 #include "../../include/gpushare_b200.h"
@@ -87,6 +88,37 @@ GSB_HD uint32_t gsb_l1_steps(uint32_t unit, uint32_t form) {
     default: return 0u;
   }
 }
+
+/* ---- gsb_test_l1_table: the twins' tables (see include/gpushare_b200.h) ---- */
+
+/* The seed whose pattern generation g of an L1_STORE table stores; generation 0 is the probe's seed, the fill. */
+GSB_HD uint32_t gsb_l1_table_seed(uint32_t seed, uint32_t g) { return seed ^ g * GSB_PAT_K0; }
+
+/* The fields of one L1_STORE table entry (GSB_L1_STORE_ENTRY); width 0: no store. */
+GSB_HD uint32_t gsb_l1_entry_word(uint32_t e) { return e & ((1u << GSB_L1_STORE_WORD_BITS) - 1u); }
+GSB_HD uint32_t gsb_l1_entry_lo(uint32_t e) { return e >> GSB_L1_STORE_WORD_BITS & 15u; }
+GSB_HD uint32_t gsb_l1_entry_width(uint32_t e) {
+  const uint32_t c = e >> (GSB_L1_STORE_WORD_BITS + 4) & 7u;
+  return c ? 1u << (c - 1u) : 0u;
+}
+GSB_HD uint32_t gsb_l1_entry_gen(uint32_t e) { return e >> 24; }
+
+/* Words of each CTA's region a table of `unit` reads: set by the case for the buffer units, fixed otherwise. */
+GSB_HD uint32_t gsb_l1_table_fixed_words(uint32_t unit) {
+  return unit == GSB_L1_UNIT_TEX ? GSB_L1_REGION_WORDS
+         : unit == GSB_L1_UNIT_CONST ? GSB_L1_CONST_WORDS
+         : unit == GSB_L1_UNIT_PARAM ? GSB_L1_PARAM_WORDS
+                                     : 0u;
+}
+
+/* uint32 expected entries per CTA a table of `unit` takes: L1_STORE 4 per region word, TEX 2 per read, none else. */
+GSB_HD uint64_t gsb_l1_table_expected_per_cta(uint32_t unit, uint64_t n, uint32_t region_words) {
+  return unit == GSB_L1_UNIT_L1_STORE ? 4ull * region_words : unit == GSB_L1_UNIT_TEX ? n : 0ull;
+}
+
+/* Host: whether gsb_test_l1_table takes this table (every refusal that needs no device; gsb_l1.cc). */
+bool gsb_l1_table_valid(uint32_t unit, const uint32_t *table, size_t n, const uint32_t *expected, size_t n_expected,
+                        uint32_t region_words);
 
 /* Indices the corrupt hook accepts for `unit` (see gsb_test_l1_corrupt). */
 GSB_HD uint32_t gsb_l1_hook_words(uint32_t unit) {

@@ -4,8 +4,8 @@
  * path, the texture unit, the constant bank, the kernel parameters) and compare each with the word computed in
  * registers (gsb_pattern.h). Host code lives in gsb_device.cu (the probe) and gsb_l1.cc (schedule, verdict, text).
  *
- * Every global load and store is inline PTX with its cache operator spelled out, so build flags cannot change which
- * path a word takes. Nothing here assumes one CTA per SM, a honoured carveout or a load that hits: a CTA reads only
+ * The instruction bodies live in gsb_l1_isa.inc, which the test-only twins l1_from_table<UNIT> (l1_table_sm90a.cu)
+ * compile from too. Nothing here assumes one CTA per SM, a honoured carveout or a load that hits: a CTA reads only
  * its own region and its own stores, so the answers stay exact whatever shares the SM; only coverage and the hit
  * ratio fall. Thread 0 of each CTA sets bit %smid of the launch's coverage bitmap.
  */
@@ -26,100 +26,9 @@ struct gsb_l1_param {
 };
 static_assert(sizeof(gsb_l1_param) == 32000, "the PARAM unit's parameter is 32000 bytes");
 
-__device__ __forceinline__ uint32_t smid() {
-  uint32_t s;
-  asm volatile("mov.u32 %0, %%smid;" : "=r"(s));
-  return s;
-}
-
-__device__ __forceinline__ uint4 ld_ca(const uint4 *p) {
-  uint4 v;
-  asm volatile("ld.global.ca.v4.u32 {%0, %1, %2, %3}, [%4];" : "=r"(v.x), "=r"(v.y), "=r"(v.z), "=r"(v.w) : "l"(p));
-  return v;
-}
-__device__ __forceinline__ uint4 ld_plain(const uint4 *p) {
-  uint4 v;
-  asm volatile("ld.global.v4.u32 {%0, %1, %2, %3}, [%4];" : "=r"(v.x), "=r"(v.y), "=r"(v.z), "=r"(v.w) : "l"(p));
-  return v;
-}
-__device__ __forceinline__ uint4 ld_evict_last(const uint4 *p) {
-  uint4 v;
-  asm volatile("ld.global.L1::evict_last.v4.u32 {%0, %1, %2, %3}, [%4];"
-               : "=r"(v.x), "=r"(v.y), "=r"(v.z), "=r"(v.w) : "l"(p));
-  return v;
-}
-__device__ __forceinline__ uint4 ld_nc(const uint4 *p) {
-  uint4 v;
-  asm volatile("ld.global.nc.v4.u32 {%0, %1, %2, %3}, [%4];" : "=r"(v.x), "=r"(v.y), "=r"(v.z), "=r"(v.w) : "l"(p));
-  return v;
-}
-
-__device__ __forceinline__ uint4 pattern(uint64_t w, uint32_t key) {
-  uint32_t l[4];
-  gsb_pattern_word(w, key, l);
-  return make_uint4(l[0], l[1], l[2], l[3]);
-}
-
-__device__ __forceinline__ uint32_t diff_bits(const uint4 &e, const uint4 &o) {
-  return __popc(e.x ^ o.x) + __popc(e.y ^ o.y) + __popc(e.z ^ o.z) + __popc(e.w ^ o.w);
-}
-
-// `words` wrong words of `bits` flipped bits on SM sm
-__device__ __forceinline__ void tally(gsb_l1_log *log, uint32_t sm, uint32_t words, uint32_t bits) {
-  atomicAdd(&log->mismatch_words, (unsigned long long)words);
-  atomicAdd(&log->mismatch_bits, (unsigned long long)bits);
-  if (sm < GSB_SM_MAX) atomicOr(&log->faulty[sm >> 5], 1u << (sm & 31u));
-}
-
-// one wrong word's record while the log has room; `w`: the expected word's index
-__device__ __forceinline__ void record(gsb_l1_log *log, uint32_t sm, uint32_t unit, uint32_t form, uint64_t w,
-                                       const uint4 &e, const uint4 &o) {
-  const unsigned slot = atomicAdd(&log->count, 1u);
-  if (slot < GSB_L1_RECORDS) {
-    gsb_l1_record &r = log->rec[slot];
-    r.smid = sm;
-    r.unit = unit;
-    r.form = form;
-    r.offset = w << 4;
-    r.expected[0] = e.x, r.expected[1] = e.y, r.expected[2] = e.z, r.expected[3] = e.w;
-    r.observed[0] = o.x, r.observed[1] = o.y, r.observed[2] = o.z, r.observed[3] = o.w;
-  }
-}
-
-// One observed word: the test hook's XOR (when `hook`), then the bit-exact compare. Returns the words compared (1).
-__device__ __forceinline__ uint32_t check(const gsb_l1_args &a, uint32_t sm, uint32_t unit, uint32_t form, uint64_t w,
-                                          uint4 e, uint4 o, bool hook) {
-  if (hook) {
-    o.x ^= (uint32_t)a.hook_xr;
-    o.y ^= (uint32_t)(a.hook_xr >> 32);
-  }
-  const uint32_t bits = diff_bits(e, o);
-  if (bits) {
-    tally(a.log, sm, 1, bits);
-    record(a.log, sm, unit, form, w, e, o);
-  }
-  return 1u;
-}
-
-// words compared by the calling thread, summed per warp (every thread of the warp calls it)
-__device__ __forceinline__ void add_words(gsb_l1_log *log, uint32_t n) {
-  n = __reduce_add_sync(0xFFFFFFFFu, n);
-  if ((threadIdx.x & 31u) == 0) atomicAdd(&log->words, (unsigned long long)n);
-}
-
-__device__ __forceinline__ void begin(const gsb_l1_args &a, uint32_t sm) {
-  if (threadIdx.x == 0 && sm < GSB_SM_MAX) atomicOr(&a.log->covered[sm >> 5], 1u << (sm & 31u));
-}
+#include "gsb_l1_isa.inc"
 
 // ---- L1_LOAD and NC: every pass over the region with one load form, timed per pass ----------------------------------
-template <uint32_t FORM>
-__device__ __forceinline__ uint4 load(const uint4 *p) {
-  if (FORM == GSB_L1_FORM_CA) return ld_ca(p);
-  if (FORM == GSB_L1_FORM_PLAIN) return ld_plain(p);
-  if (FORM == GSB_L1_FORM_EVICT_LAST) return ld_evict_last(p);
-  return ld_nc(p);
-}
-
 template <uint32_t UNIT, uint32_t FORM>
 __device__ __forceinline__ uint32_t passes(const gsb_l1_args &a, uint32_t sm, uint32_t key) {
   const uint32_t t = threadIdx.x, form = UNIT == GSB_L1_UNIT_NC ? 0u : FORM;
@@ -165,28 +74,10 @@ __global__ void __launch_bounds__(GSB_L1_THREADS, 1) l1_nc(const gsb_l1_args a) 
 }
 
 // ---- L1_STORE: lines made resident, partial stores from another warp, read back through L1 -------------------------
-__device__ __forceinline__ uint32_t pick(const uint4 &v, uint32_t lane) {
-  return lane == 0 ? v.x : lane == 1 ? v.y : lane == 2 ? v.z : v.w;
-}
-
 __device__ __forceinline__ void store(uint4 *word, uint64_t w, uint32_t key2) {
   uint32_t lo, width;
   gsb_l1_store_span(w, &lo, &width);
-  const uint4 g = pattern(w, key2);
-  char *p = reinterpret_cast<char *>(word) + lo;
-  const uint32_t lane = pick(g, lo >> 2);
-  switch (width) {
-    case 1: asm volatile("st.global.u8 [%0], %1;" ::"l"(p), "r"(lane >> (8 * (lo & 3u))) : "memory"); break;
-    case 2: asm volatile("st.global.u16 [%0], %1;" ::"l"(p), "r"(lane >> (8 * (lo & 3u))) : "memory"); break;
-    case 4: asm volatile("st.global.u32 [%0], %1;" ::"l"(p), "r"(lane) : "memory"); break;
-    case 8:
-      asm volatile("st.global.v2.u32 [%0], {%1, %2};" ::"l"(p), "r"(lane), "r"(pick(g, (lo >> 2) + 1u)) : "memory");
-      break;
-    default:
-      asm volatile("st.global.v4.u32 [%0], {%1, %2, %3, %4};" ::"l"(p), "r"(g.x), "r"(g.y), "r"(g.z), "r"(g.w)
-                   : "memory");
-      break;
-  }
+  store_bytes(word, lo, width, pattern(w, key2));
 }
 
 __global__ void __launch_bounds__(GSB_L1_THREADS, 1) l1_store(const gsb_l1_args a) {

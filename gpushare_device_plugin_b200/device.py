@@ -953,8 +953,25 @@ def test_l1_skip(idx: int, smid: int) -> None:
     check(lib.gsb_test_l1_skip(idx, smid), f"gsb_test_l1_skip({idx})")
 
 
+def test_l1_table(idx: int, unit: int, table, expected=None, region_words: int = 0) -> None:
+    """Test hook: the next L1 probe of `idx` that runs `unit` runs its test-only twin on `table` (uint32 entries, as
+    gsb_test_l1_table lays them out) against `expected` (L1_STORE: the region words after the last round, every CTA's;
+    TEX: the texel each read returns, -1 for 0), with CTA regions of `region_words` words; once. table=None disarms
+    it."""
+    import numpy as np
+    if table is None:
+        check(lib.gsb_test_l1_table(idx, unit, None, 0, None, 0, 0), f"gsb_test_l1_table({idx})")
+        return
+    t = np.ascontiguousarray(np.asarray(table).astype(np.uint32))
+    e = None if expected is None else np.ascontiguousarray(np.asarray(expected).astype(np.int64).astype(np.uint32))
+    ptr = lambda x: None if x is None else x.ctypes.data_as(C.POINTER(C.c_uint32))  # noqa: E731
+    check(lib.gsb_test_l1_table(idx, unit, ptr(t), len(t), ptr(e), 0 if e is None else len(e), region_words),
+          f"gsb_test_l1_table({idx})")
+
+
 test_l1_corrupt.__test__ = False
 test_l1_skip.__test__ = False
+test_l1_table.__test__ = False
 
 
 def fault_classify(offset: int, expected, observed) -> FaultRecord:

@@ -1738,6 +1738,49 @@ int gsb_test_l1_corrupt(uint32_t idx, uint32_t smid, uint32_t unit, uint32_t ind
  * so every word it owed reads back as generation 1 (STALE). Refused before any device is touched when smid is out of
  * range. */
 int gsb_test_l1_skip(uint32_t idx, uint32_t smid);
+/* gsb_test_l1_table: table sizes, the L1_STORE entry and flags, the TEX 1-D marker */
+#define GSB_L1_TABLE_MAX (1u << 20)           /* uint32 table entries */
+#define GSB_L1_TABLE_EXPECTED_MAX (1u << 24)  /* uint32 expected entries */
+#define GSB_L1_TABLE_REGION_MAX 131072u       /* words of a buffer unit's region per CTA: 2 MiB */
+#define GSB_L1_TABLE_ROUNDS_MAX 8u            /* L1_STORE rounds */
+#define GSB_L1_STORE_WORD_BITS 17
+/* one L1_STORE table entry: thread's store of generation gen (1..255) over bytes [lo, lo + (1 << width_log2)) of
+ * region word `word`; 0 = no store */
+#define GSB_L1_STORE_ENTRY(word, lo, width_log2, gen) \
+  ((uint32_t)(word) | (uint32_t)(lo) << 17 | ((uint32_t)(width_log2) + 1u) << 21 | (uint32_t)(gen) << 24)
+#define GSB_L1_TABLE_RESIDENT 1u /* L1_STORE: read the whole region through L1 before the first round */
+#define GSB_L1_TABLE_READ_OWN 2u /* L1_STORE: each writer reads its word back right after its store, no barrier */
+#define GSB_L1_TEX_1D 0x80000000u /* TEX: a read whose y is this is tex1Dfetch of region word x */
+/* test hook: the next gsb_l1_probe of device idx that runs `unit` runs the unit's test-only twin on the chosen reads of
+ * `table` (n uint32 entries) instead of the shipped schedule, in every launch of the unit; once. Every CTA c reads its
+ * own region of `region_words` words (c * region_words onward), which the FILL launch fills with the seed's pattern:
+ *   L1_LOAD, NC  table[p * region_words + k * GSB_L1_THREADS + t]: the region word thread t reads at step k of pass p
+ *                (n / region_words passes, each timed as the shipped passes are; L1_LOAD runs the table once with each
+ *                of its three load forms); the expected word is computed on the SM. region_words: a multiple of
+ *                GSB_L1_THREADS up to GSB_L1_TABLE_REGION_MAX.
+ *   L1_STORE     table[0]: GSB_L1_TABLE_* flags; table[1 + r * GSB_L1_THREADS + t]: thread t's store in round r
+ *                (GSB_L1_STORE_ENTRY or 0), rounds separated by bar.sync; the value is generation gen's pattern word
+ *                of the region word's index. After the last round every word is read back through L1 (form 1) and
+ *                compared on the SM with expected[(c * region_words + w) * 4 + lane]; a read of the resident pass is
+ *                form 0, a writer's own read-back form 2 (its stored bytes only). region_words as for L1_LOAD, at
+ *                most 2^GSB_L1_STORE_WORD_BITS.
+ *   TEX          (table[2 r], table[2 r + 1]) = (x, y) of read r = k * GSB_L1_THREADS + t: with y = GSB_L1_TEX_1D,
+ *                tex1Dfetch of region word x (form 0); else the 2-D reads at texel (x, c * GSB_L1_TEX_ROWS + y) with
+ *                clamp (form 1) and border addressing (form 2). expected[(c * n / 2 + r) * 2 + {0, 1}]: the buffer word
+ *                each returns (form 0: slot 0), as int32, -1 for a border read that returns 0. region_words:
+ *                GSB_L1_REGION_WORDS.
+ *   CONST, PARAM table[k * GSB_L1_THREADS + t]: the bank's or the parameter's word thread t reads at step k (form 1).
+ *                region_words: GSB_L1_CONST_WORDS or GSB_L1_PARAM_WORDS.
+ * The table and the expected words take their share of the probe's transient buffer. gsb_test_l1_skip applies to an
+ * L1_STORE twin too: the CTA on that SM stores nothing in the last round. table == NULL disarms the unit. Refused
+ * before any device is touched: an unknown unit; n or n_expected past GSB_L1_TABLE_MAX or GSB_L1_TABLE_EXPECTED_MAX,
+ * not a whole number of steps, passes or rounds, or n_expected not a whole number of CTAs; a region size the unit does
+ * not take; an index outside the CTA's region, the bank or the parameter; unknown flags; a store that is misaligned,
+ * wider than 16 bytes, past the word or of generation 0; two stores to the same byte in one round; a TEX coordinate
+ * of magnitude 2^21 or more, a 1-D index outside the region, an expected texel below -1. n_expected other than the
+ * device's sm_count CTAs is refused once the device is known. */
+int gsb_test_l1_table(uint32_t idx, uint32_t unit, const uint32_t *table, size_t n, const uint32_t *expected,
+                      size_t n_expected, uint32_t region_words);
 
 /* ---- Allocate (a12, a13): wire bytes in, wire bytes out ---------------------------------- */
 

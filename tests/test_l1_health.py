@@ -568,3 +568,12 @@ def test_the_kernels_are_a_module_of_their_own_loaded_by_the_library():
     assert "l1_check_sm90a_cu" not in main
     needed = subprocess.run(["readelf", "-d", _abi.LIB_PATH], capture_output=True, text=True, check=True).stdout
     assert "[libgpushare_b200_l1.so]" in needed and "$ORIGIN" in needed
+    # its launch entry points: the shipped kernels', the bank's, occupancy, preload, and the twins' (gsb_test_l1_table,
+    # their own translation unit l1_table_sm90a.cu)
+    syms = subprocess.run(["nm", "-D", "--defined-only", _abi.L1_LIB_PATH], capture_output=True, text=True,
+                          check=True).stdout
+    assert sorted(m[1][:int(m[0])] for m in re.findall(r"_Z(\d+)(gsb_\w+)", syms)) == [
+        "gsb_l1_const_upload", "gsb_l1_kernel_launch", "gsb_l1_kernel_preload", "gsb_l1_occupancy", "gsb_l1_table_launch"]
+    main_syms = subprocess.run(["nm", "-D", "--defined-only", _abi.LIB_PATH], capture_output=True, text=True,
+                               check=True).stdout
+    assert "gsb_l1_table_launch" not in main_syms and "gsb_test_l1_table" in main_syms

@@ -257,16 +257,16 @@ def test_new_entry_points_are_declared_and_bound():
 
 # ---- the twins and the shipped kernels ------------------------------------------------------------------------------
 
-def _cuobjdump(*args):
+def _cuobjdump(*args, lib=None):
     tool = shutil.which("cuobjdump") or "/usr/local/cuda/bin/cuobjdump"
     if not os.access(tool, os.X_OK):
         pytest.skip("cuobjdump not available")
-    return subprocess.run([tool, *args, _abi.LIB_PATH], capture_output=True, text=True, check=True).stdout
+    return subprocess.run([tool, *args, lib or _abi.LIB_PATH], capture_output=True, text=True, check=True).stdout
 
 
-def _sass_functions():
+def _sass_functions(lib=None):
     fns, name = {}, None
-    for line in _cuobjdump("-sass").splitlines():
+    for line in _cuobjdump("-sass", lib=lib).splitlines():
         if "Function :" in line:
             name = line.split("Function :", 1)[1].strip()
             fns[name] = []
@@ -331,9 +331,9 @@ def test_stable_name_drops_only_the_anonymous_namespace_hash():
 
 
 def test_shipped_kernels_compile_to_the_recorded_sass():
-    """every kernel the library shipped before the twins keeps its instruction words (tests/golden: sha256 of each
-    function's cuobjdump -sass lines by stable_name, recorded with the nvcc release named there), wherever the tree
-    was built"""
+    """every kernel the library and its L1 module shipped before the twins keeps its instruction words (tests/golden:
+    sha256 of each function's cuobjdump -sass lines by stable_name, recorded with the nvcc release named there),
+    wherever the tree was built"""
     golden = json.load(open(os.path.join(ROOT, "tests", "golden", "shipped_kernels_sass.json")))
     nvcc = shutil.which("nvcc") or "/usr/local/cuda/bin/nvcc"
     if not os.access(nvcc, os.X_OK):
@@ -342,12 +342,16 @@ def test_shipped_kernels_compile_to_the_recorded_sass():
     if release != golden["nvcc"]:
         pytest.skip(f"recorded with {golden['nvcc']}, this build uses {release}")
     fns = _sass_functions()
+    l1 = _sass_functions(_abi.L1_LIB_PATH)
+    assert not set(fns) & set(l1)
+    fns.update(l1)
     got = {stable_name(n): hashlib.sha256("\n".join(b).encode()).hexdigest() for n, b in fns.items()}
     assert len(got) == len(fns)
     changed = [n for n, h in golden["kernels"].items() if got.get(n) != h]
     assert not changed, changed
-    assert sorted(set(got) - set(golden["kernels"])) == sorted(n for n in got if "sfu_from_table" in n)
+    assert sorted(set(got) - set(golden["kernels"])) == sorted(n for n in got if re.search(r"(sfu|l1)_from_table", n))
     assert sum("sfu_check" in n for n in golden["kernels"]) == 6
+    assert sum("l1_check" in n for n in golden["kernels"]) == 6
 
 
 # ---- the pure models in every floating-point environment ------------------------------------------------------------
