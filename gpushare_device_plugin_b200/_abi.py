@@ -14,6 +14,8 @@ _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(_HERE, "libgpushare_b200.so")
 # the L1 and constant-cache check's kernels, a module of their own that LIB_PATH loads
 L1_LIB_PATH = os.path.join(_HERE, "libgpushare_b200_l1.so")
+# the memory-ordering check's kernel, likewise a module of its own that LIB_PATH loads
+ORDER_LIB_PATH = os.path.join(_HERE, "libgpushare_b200_order.so")
 
 GSB_UUID_BUFFER_SIZE = 80
 GSB_BUSID_BUFFER_SIZE = 32
@@ -105,6 +107,18 @@ GSB_L1_RECORDS, GSB_L1_MAX_LAUNCHES, GSB_L1_FORMS = 64, 3, 4
 GSB_L1_ZERO_TEXEL = (1 << 63) - 1
 GSB_L1_CORRUPT, GSB_L1_FAILED = 1, 2
 L1_CONDITION_NAMES = {1: "wrong word through L1, texture or constant cache", 2: "L1 probe failed"}
+GSB_ORDER_UNIT_MP_RELACQ, GSB_ORDER_UNIT_MP_FENCE, GSB_ORDER_UNIT_SB_SC, GSB_ORDER_UNIT_IRIW_SC, GSB_ORDER_UNIT_CORR, \
+    GSB_ORDER_UNIT_MP_RELAXED = range(6)
+ORDER_UNIT_NAMES = ["mp_relacq", "mp_fence", "sb_sc", "iriw_sc", "corr", "mp_relaxed"]
+GSB_ORDER_UNITS, GSB_ORDER_DISTANCES, GSB_ORDER_THREADS, GSB_ORDER_OBS_DEFAULT, GSB_ORDER_OBS_MAX, GSB_ORDER_WORDS, \
+    GSB_ORDER_RECORDS = 6, 3, 256, 1024, 65536, 5, 64
+GSB_ORDER_WAIT_NS, GSB_ORDER_WAIT_NS_PER_OBS = 100000000, 5000
+GSB_ORDER_CLS_ALLOWED, GSB_ORDER_CLS_OVERLAP, GSB_ORDER_CLS_WEAK, GSB_ORDER_CLS_FORBIDDEN, GSB_ORDER_CLS_CORRUPT, \
+    GSB_ORDER_CLS_LOST = range(6)
+GSB_ORDER_CORRUPT, GSB_ORDER_FORBIDDEN, GSB_ORDER_LOST, GSB_ORDER_TIMEOUT, GSB_ORDER_FAILED = 1, 2, 4, 8, 16
+ORDER_CONDITION_NAMES = {1: "word read back that no writer stored", 2: "outcome the memory model forbids",
+                         4: "store lost after the grid barrier", 8: "grid barrier ran out",
+                         16: "memory-ordering probe failed"}
 # gsb_test_l1_table
 GSB_L1_TABLE_MAX, GSB_L1_TABLE_EXPECTED_MAX, GSB_L1_TABLE_REGION_MAX, GSB_L1_TABLE_ROUNDS_MAX = 1 << 20, 1 << 24, 131072, 8
 GSB_L1_STORE_WORD_BITS, GSB_L1_TABLE_RESIDENT, GSB_L1_TABLE_READ_OWN, GSB_L1_TEX_1D = 17, 1, 2, 0x80000000
@@ -121,8 +135,8 @@ GSB_VARIANT_AUTO, GSB_VARIANT_DIRECT, GSB_VARIANT_CPASYNC, GSB_VARIANT_BULK, GSB
 VARIANT_NAMES = {0: "auto", 1: "direct", 2: "cpasync", 3: "bulk", 4: "bulkw", 5: "bulkd"}
 GSB_PROBE_TIMED, GSB_PROBE_SEED_TABLE = 1, 2
 GSB_EVENT_XID, GSB_EVENT_PROBE, GSB_EVENT_INVENTORY, GSB_EVENT_ECC, GSB_EVENT_LINK, GSB_EVENT_COPY, GSB_EVENT_SM, \
-    GSB_EVENT_CLUSTER, GSB_EVENT_ATOMIC, GSB_EVENT_TENSOR, GSB_EVENT_SFU, GSB_EVENT_L1 = 8, 0x100, 0x200, 0x400, 0x800, \
-    0x1000, 0x2000, 0x4000, 0x8000, 0x10000, 0x20000, 0x40000
+    GSB_EVENT_CLUSTER, GSB_EVENT_ATOMIC, GSB_EVENT_TENSOR, GSB_EVENT_SFU, GSB_EVENT_L1, GSB_EVENT_ORDER = 8, 0x100, 0x200, \
+    0x400, 0x800, 0x1000, 0x2000, 0x4000, 0x8000, 0x10000, 0x20000, 0x40000, 0x80000
 GSB_PROBE_FAULT_MISMATCH, GSB_PROBE_FAULT_LAUNCH, GSB_PROBE_RECOVERED, GSB_PROBE_FAULT_WEDGED = 1, 2, 3, 4
 GSB_INVENTORY_IDENTITY_CHANGED, GSB_INVENTORY_TOTAL_CHANGED = 1, 2
 GSB_ECC_VALID_MODE, GSB_ECC_VALID_VOLATILE, GSB_ECC_VALID_AGGREGATE, GSB_ECC_VALID_DRAM, GSB_ECC_VALID_REMAP, \
@@ -141,7 +155,7 @@ GSB_OPT_INVENTORY_POLICY, GSB_OPT_WAIT_SPIN_US, GSB_OPT_WATCHDOG_MS, GSB_OPT_INV
     GSB_OPT_TRANSIENT_KEEP_FREE_BYTES, GSB_OPT_SWEEP_EVERY_CYCLES, GSB_OPT_ECC_HEALTH, GSB_OPT_LINK_PROBE_EVERY_CYCLES, \
     GSB_OPT_COPY_PROBE_EVERY_CYCLES, GSB_OPT_SM_PROBE_EVERY_CYCLES, GSB_OPT_CLUSTER_PROBE_EVERY_CYCLES, \
     GSB_OPT_ATOMIC_PROBE_EVERY_CYCLES, GSB_OPT_TENSOR_PROBE_EVERY_CYCLES, GSB_OPT_SFU_PROBE_EVERY_CYCLES, \
-    GSB_OPT_L1_PROBE_EVERY_CYCLES = 1, 2, 3, 4, 5, 6, 7, 8, 9, 10, 11, 12, 13, 14, 15
+    GSB_OPT_L1_PROBE_EVERY_CYCLES, GSB_OPT_ORDER_PROBE_EVERY_CYCLES = 1, 2, 3, 4, 5, 6, 7, 8, 9, 10, 11, 12, 13, 14, 15, 16
 GSB_INVENTORY_SNAPSHOT, GSB_INVENTORY_LIVE = 0, 1
 GSB_ALLOC_MATCHED, GSB_ALLOC_SINGLE_GPU, GSB_ALLOC_ERR_RESPONSE = 1, 2, 3
 UINT64_MAX = (1 << 64) - 1
@@ -175,6 +189,8 @@ SYMBOLS = [
     "gsb_sfu_text", "gsb_test_sfu_corrupt", "gsb_test_sfu_inputs",
     "gsb_l1_probe", "gsb_l1_stats_get", "gsb_l1_schedule", "gsb_l1_conditions", "gsb_l1_text", "gsb_test_l1_corrupt",
     "gsb_test_l1_skip", "gsb_test_l1_table",
+    "gsb_order_probe", "gsb_order_stats_get", "gsb_order_distance", "gsb_order_iriw_distance", "gsb_order_pairing",
+    "gsb_order_classify", "gsb_order_conditions", "gsb_order_text", "gsb_test_order_inject", "gsb_test_order_skip",
     "gsb_allocate", "gsb_allocate_err_response", "gsb_patch_assigned_body",
 ]
 
@@ -952,6 +968,75 @@ class L1Stats(C.Structure):
     ]
 
 
+class OrderCfg(C.Structure):
+    _fields_ = [
+        ("seed", C.c_uint32),
+        ("seed_expect", C.c_uint32),
+        ("units", C.c_uint32),
+        ("observations", C.c_uint32),
+    ]
+
+
+class OrderRecord(C.Structure):
+    _fields_ = [
+        ("unit", C.c_uint32),
+        ("distance", C.c_uint32),
+        ("cls", C.c_uint32),
+        ("smid", C.c_uint32),
+        ("producer", C.c_uint32 * 3),
+        ("index", C.c_uint32),
+        ("words", C.c_uint64 * GSB_ORDER_WORDS),
+    ]
+
+
+class OrderUnitResult(C.Structure):
+    _fields_ = [
+        ("status", C.c_int32),
+        ("launches", C.c_uint32),
+        ("refused", C.c_uint32),
+        ("sms_covered", C.c_uint32),
+        ("words_checked", C.c_uint64),
+        ("mismatch_words", C.c_uint64),
+        ("mismatch_bits", C.c_uint64),
+        ("corrupt", C.c_uint64),
+        ("forbidden", C.c_uint64),
+        ("lost", C.c_uint64),
+        ("timeout", C.c_uint64),
+        ("overlap", C.c_uint64),
+        ("weak", C.c_uint64),
+        ("kernel_ns", C.c_uint64),
+    ]
+
+
+class OrderResult(C.Structure):
+    _fields_ = [
+        ("status", C.c_int32),
+        ("sm_count", C.c_uint32),
+        ("seed", C.c_uint32),
+        ("seed_expect", C.c_uint32),
+        ("units", C.c_uint32),
+        ("observations", C.c_uint32),
+        ("distance", C.c_uint32 * GSB_ORDER_DISTANCES),
+        ("sms_covered", C.c_uint32),
+        ("n_records", C.c_uint32),
+        ("covered", C.c_uint32 * (GSB_SM_MAX // 32)),
+        ("faulty", C.c_uint32 * (GSB_SM_MAX // 32)),
+        ("unit", OrderUnitResult * GSB_ORDER_UNITS),
+        ("records", OrderRecord * GSB_ORDER_RECORDS),
+        ("wall_ns", C.c_uint64),
+    ]
+
+
+class OrderStats(C.Structure):
+    _fields_ = [
+        ("probes", C.c_uint64),
+        ("faults", C.c_uint64),
+        ("skipped", C.c_uint64),
+        ("incomplete", C.c_uint64),
+        ("last", OrderResult),
+    ]
+
+
 class Pod(C.Structure):
     _fields_ = [
         ("name", C.c_char_p),
@@ -1106,6 +1191,16 @@ def _load() -> C.CDLL:
         "gsb_test_l1_corrupt": (C.c_int, [C.c_uint32, C.c_uint32, C.c_uint32, C.c_uint32, C.c_uint64]),
         "gsb_test_l1_skip": (C.c_int, [C.c_uint32, C.c_uint32]),
         "gsb_test_l1_table": (C.c_int, [C.c_uint32, C.c_uint32, u32p, C.c_size_t, u32p, C.c_size_t, C.c_uint32]),
+        "gsb_order_probe": (C.c_int, [C.c_uint32, C.POINTER(OrderCfg), C.POINTER(OrderResult)]),
+        "gsb_order_stats_get": (C.c_int, [C.c_uint32, C.POINTER(OrderStats)]),
+        "gsb_order_distance": (C.c_uint32, [C.c_uint32] * 3),
+        "gsb_order_iriw_distance": (C.c_uint32, [C.c_uint32] * 2),
+        "gsb_order_pairing": (C.c_int, [C.c_uint32] * 4 + [u32p]),
+        "gsb_order_classify": (C.c_uint32, [C.c_uint32, C.c_uint32, u32p, u64p, C.c_uint32]),
+        "gsb_order_conditions": (C.c_uint32, [C.POINTER(OrderResult)]),
+        "gsb_order_text": (C.c_int64, [C.POINTER(OrderResult), C.c_char_p, C.c_char_p, C.c_size_t]),
+        "gsb_test_order_inject": (C.c_int, [C.c_uint32] * 4),
+        "gsb_test_order_skip": (C.c_int, [C.c_uint32, C.c_uint32]),
         "gsb_allocate": (C.c_int, [C.POINTER(AllocateCtx), C.POINTER(Pod), C.c_uint32, C.c_char_p, C.c_size_t, C.c_void_p, C.c_size_t, C.POINTER(C.c_size_t), C.POINTER(C.c_int32), u32p]),
         "gsb_allocate_err_response": (C.c_int, [C.POINTER(AllocateCtx), C.c_char_p, C.c_size_t, C.c_void_p, C.c_size_t, C.POINTER(C.c_size_t)]),
         "gsb_patch_assigned_body": (C.c_int, [C.c_uint64, C.c_char_p, C.c_size_t]),

@@ -164,6 +164,16 @@ const Check kChecks[] = {
      },
      {{GSB_L1_CORRUPT, "wrong word through L1, texture or constant cache"}, {GSB_L1_FAILED, "L1 probe failed"}},
      "L1 condition ?"},
+    {&Flags::probe_order_every, GSB_OPT_ORDER_PROBE_EVERY_CYCLES, GSB_EVENT_ORDER, "memory-ordering health", "order",
+     [](uint32_t i, const std::string &u) {
+       return probed<gsb_order_stats>(i, u, gsb_order_stats_get, gsb_order_text, nullptr, &gsb_order_stats::incomplete);
+     },
+     {{GSB_ORDER_CORRUPT, "word read back that no writer stored"},
+      {GSB_ORDER_FORBIDDEN, "outcome the memory model forbids"},
+      {GSB_ORDER_LOST, "store lost after the grid barrier"},
+      {GSB_ORDER_TIMEOUT, "grid barrier ran out"},
+      {GSB_ORDER_FAILED, "memory-ordering probe failed"}},
+     "memory-ordering condition ?"},
 };
 constexpr size_t kNumChecks = sizeof kChecks / sizeof kChecks[0];
 

@@ -53,6 +53,7 @@
 #include "gsb_tensor_kat.h"
 #include "gsb_sfu_kat.h"
 #include "gsb_l1.h"
+#include "gsb_order.h"
 
 namespace {
 
@@ -325,6 +326,17 @@ struct Device {
   // what the L1 probe's CONST unit copies into its bank and its PARAM unit passes as its parameter: the copy is
   // asynchronous, so its source lives as long as the device
   std::vector<uint4> l1_const, l1_param;
+  // memory-ordering health: gsb_test_order_inject by GSB_ORDER_UNIT_*, gsb_test_order_skip
+  struct OrderInject {
+    bool armed = false;
+    uint32_t smid = 0, index = 0;
+  };
+  struct OrderHooks {
+    std::array<OrderInject, GSB_ORDER_UNITS> inject;
+    bool skip_armed = false;
+    uint32_t skip_smid = 0;
+  };
+  CheckState<gsb_order_stats, OrderHooks> order;
 
   // persistent worker (gsb_cycle_all / gsb_probe_all): one host thread per device
   std::thread worker;
@@ -354,7 +366,7 @@ struct Global {
   std::atomic<uint64_t> transient_keep_free{1ull << 30};
   std::atomic<uint64_t> sweep_every{0};
   std::atomic<uint64_t> ecc_health{0};
-  std::atomic<uint64_t> check_every[8] = {};  // GSB_OPT_*_PROBE_EVERY_CYCLES, by the check's place in Checks
+  std::atomic<uint64_t> check_every[9] = {};  // GSB_OPT_*_PROBE_EVERY_CYCLES, by the check's place in Checks
 
   // one link or copy probe's pinned buffers at a time in the whole process (the DaemonSet's memory limit covers 8 GPUs)
   std::mutex link_mu;
@@ -556,6 +568,7 @@ int ensure_ready(Device *d) {
   if (pe == cudaSuccess) pe = (cudaError_t)gsb_sfu_kernel_preload(smem_optin);
   if (pe == cudaSuccess) pe = (cudaError_t)gsb_l1_kernel_preload();
   if (pe == cudaSuccess) pe = (cudaError_t)gsb_sfu_operands_preload(smem_optin);
+  if (pe == cudaSuccess) pe = (cudaError_t)gsb_order_kernel_preload(smem_optin);
   if (pe != cudaSuccess) {
     set_error("loading the probe kernels on %s: %s", d->uuid, cudaGetErrorString(pe));
     return (pe == cudaErrorInvalidDeviceFunction || pe == cudaErrorNoKernelImageForDevice) ? GSB_ERR_UNSUPPORTED_ARCH
@@ -3343,6 +3356,112 @@ int l1_probe_locked(Device *d, const gsb_l1_cfg *cfg, gsb_l1_result *out) {
   return rc;
 }
 
+// ------------------------------------------------------------------ memory-ordering health
+
+constexpr uint32_t kOrderAllUnits = (1u << GSB_ORDER_UNITS) - 1;
+
+int order_probe_locked(Device *d, const gsb_order_cfg *cfg, gsb_order_result *out) {
+  const uint64_t t0 = now_ns();
+  if (cfg->units & ~kOrderAllUnits || cfg->observations > GSB_ORDER_OBS_MAX) {
+    set_error("invalid memory-ordering probe configuration (units 0x%x, observations %u)", cfg->units,
+              cfg->observations);
+    return out->status = GSB_ERR_INVALID_ARGUMENT;
+  }
+  out->units = cfg->units ? cfg->units : kOrderAllUnits;
+  out->observations = cfg->observations ? cfg->observations : GSB_ORDER_OBS_DEFAULT;
+  out->sm_count = d->sm_count;
+  int rc = ensure_ready(d);
+  if (!rc) rc = sm_drain_kept_locked(d);
+  if (rc) return out->status = rc;
+  out->seed = seed_or_fresh(cfg->seed, 0x4F520000u, &d->order.seed);
+  out->seed_expect = cfg->seed_expect ? cfg->seed_expect : out->seed;
+  const Device::OrderHooks hooks = take_hooks(d, &d->order.hooks);
+  const uint32_t n = d->sm_count, m = out->observations;
+  for (uint32_t k = 0; k < GSB_ORDER_DISTANCES; k++) out->distance[k] = gsb_order_distance_of(k, n, out->seed);
+  // one transient buffer: the launch log, every CTA's locations and scratch region, the published observations and
+  // the ranks' %smid, each 256-byte aligned
+  const auto align = [](size_t x) { return (x + 255) / 256 * 256; };
+  const size_t locs_off = align(sizeof(gsb_order_log)), scratch_off = locs_off + (size_t)n * GSB_ORDER_LOC_WORDS * 8;
+  const size_t obs_off = scratch_off + (size_t)n * GSB_ORDER_SCRATCH_WORDS * 16;
+  const size_t smid_off = obs_off + align((size_t)n * m * GSB_ORDER_OBS_WORDS * 8);
+  SmBuffer buf(d, rc);
+  rc = buf.alloc("memory-ordering probe", smid_off + align((size_t)n * sizeof(uint32_t)));
+  char *const base = static_cast<char *>(buf.p);
+  int smem = 0;
+  if (rc == GSB_OK) rc = smem_optin_locked(d, &smem);
+  gsb_order_args a;
+  memset(&a, 0, sizeof a);
+  a.log = reinterpret_cast<gsb_order_log *>(base);
+  a.locs = reinterpret_cast<unsigned long long *>(base + locs_off);
+  a.scratch = reinterpret_cast<uint4 *>(base + scratch_off);
+  a.obs = reinterpret_cast<unsigned long long *>(base + obs_off);
+  a.smids = reinterpret_cast<uint32_t *>(base + smid_off);
+  a.seed = out->seed;
+  a.seed_expect = out->seed_expect;
+  a.observations = m;
+  a.smem_bytes = (uint32_t)smem;
+  bool first = true;
+  for (uint32_t u = 0; u < GSB_ORDER_UNITS && rc == GSB_OK; u++) {
+    if (!(out->units >> u & 1u)) continue;
+    gsb_order_unit_result &ur = out->unit[u];
+    uint32_t unit_cov[GSB_SM_MAX / 32] = {0};
+    for (uint32_t k = 0; k < GSB_ORDER_DISTANCES; k++) {
+      a.unit = u;
+      a.distance = out->distance[k];
+      a.dist_index = k;
+      // test hooks: the unit's first launch only
+      a.inject_smid = k == 0 && hooks.inject[u].armed ? hooks.inject[u].smid : GSB_SM_MAX;
+      a.inject_index = hooks.inject[u].index;
+      a.skip_smid = k == 0 && u == GSB_ORDER_UNIT_MP_RELACQ && hooks.skip_armed ? hooks.skip_smid : GSB_SM_MAX;
+      bool refused = false;
+      gsb_order_log log;
+      const int lrc = sm_launch_locked(
+          d, "memory-ordering check",
+          [&] {
+            const int e = gsb_order_kernel_launch(n, &a, d->stream);
+            if (e != (int)cudaErrorCooperativeLaunchTooLarge) return e;
+            refused = true;  // the CTAs cannot all be resident at once: the launch is skipped, not failed
+            return (int)cudaSuccess;
+          },
+          a.log, &log, sizeof log, (GSB_ORDER_WAIT_NS + gsb_order_wait_ns(m)) / 1000000ull, nullptr, &ur.kernel_ns);
+      if (lrc != GSB_OK) {
+        ur.status = rc = lrc;
+        break;
+      }
+      if (refused) {
+        ur.refused++;
+        continue;
+      }
+      uint32_t covered[GSB_SM_MAX / 32] = {0};
+      fold_log(log, &ur, out, covered);
+      ur.corrupt += log.corrupt;
+      ur.forbidden += log.forbidden;
+      ur.lost += log.lost;
+      ur.timeout += log.timeout;
+      ur.overlap += log.overlap;
+      ur.weak += log.weak;
+      for (int i = 0; i < GSB_SM_MAX / 32; i++) unit_cov[i] = ur.launches ? unit_cov[i] & covered[i] : covered[i];
+      ur.launches++;
+    }
+    if (!ur.launches) continue;
+    ur.sms_covered = popcount_bitmap(unit_cov);
+    for (int i = 0; i < GSB_SM_MAX / 32; i++) out->covered[i] = first ? unit_cov[i] : out->covered[i] & unit_cov[i];
+    first = false;
+  }
+  out->sms_covered = popcount_bitmap(out->covered);
+  buf.release();
+  out->wall_ns = now_ns() - t0;
+  out->status = rc;
+  bool ran = false, short_cover = false;
+  for (const gsb_order_unit_result &ur : out->unit) {
+    ran = ran || ur.launches != 0;
+    short_cover = short_cover || ur.refused != 0 || (ur.launches != 0 && ur.status == GSB_OK && ur.sms_covered < n);
+  }
+  count_probe(d, &d->order.stats, *out, ran, gsb_order_conditions(out),
+              short_cover ? &d->order.stats.incomplete : nullptr);
+  return rc;
+}
+
 // ------------------------------------------------------------------ the periodic checks, described once
 
 template <typename Run>
@@ -3376,8 +3495,11 @@ using TensorCheck = Check<GSB_OPT_TENSOR_PROBE_EVERY_CYCLES, GSB_EVENT_TENSOR, &
                           &gsb_tensor_conditions>;
 using SfuCheck = Check<GSB_OPT_SFU_PROBE_EVERY_CYCLES, GSB_EVENT_SFU, &Device::sfu, &sfu_probe_locked, &gsb_sfu_conditions>;
 using L1Check = Check<GSB_OPT_L1_PROBE_EVERY_CYCLES, GSB_EVENT_L1, &Device::l1, &l1_probe_locked, &gsb_l1_conditions>;
+using OrderCheck = Check<GSB_OPT_ORDER_PROBE_EVERY_CYCLES, GSB_EVENT_ORDER, &Device::order, &order_probe_locked,
+                         &gsb_order_conditions>;
 // in the order the prober runs them when several are due after the same cycle; G.check_every follows it
-using Checks = std::tuple<LinkCheck, CopyCheck, SmCheck, ClusterCheck, AtomicCheck, TensorCheck, SfuCheck, L1Check>;
+using Checks =
+    std::tuple<LinkCheck, CopyCheck, SmCheck, ClusterCheck, AtomicCheck, TensorCheck, SfuCheck, L1Check, OrderCheck>;
 static_assert(std::tuple_size<Checks>::value == std::extent<decltype(G.check_every)>::value, "one cadence per check");
 
 // f(check, its place in Checks) for every periodic check, in order
@@ -4299,6 +4421,42 @@ int gsb_test_l1_skip(uint32_t idx, uint32_t smid) {
   std::lock_guard<std::mutex> lk(d->smu);
   d->l1.hooks.skip_armed = true;
   d->l1.hooks.skip_smid = smid;
+  return GSB_OK;
+}
+
+int gsb_order_probe(uint32_t idx, const gsb_order_cfg *cfg, gsb_order_result *out) {
+  // a bad configuration is refused before any device is touched
+  return probe_entry(idx, cfg, out, &OrderCheck::run, [](const gsb_order_cfg *c, gsb_order_result *) {
+    return c->units & ~kOrderAllUnits || c->observations > GSB_ORDER_OBS_MAX ? GSB_ERR_INVALID_ARGUMENT : GSB_OK;
+  });
+}
+
+int gsb_order_stats_get(uint32_t idx, gsb_order_stats *out) {
+  return stats_entry(idx, out, [](Device *d) { return &d->order.stats; });
+}
+
+int gsb_test_order_inject(uint32_t idx, uint32_t smid, uint32_t unit, uint32_t index) {
+  std::shared_lock<std::shared_mutex> api_lk(G.api_mu);
+  if (unit >= GSB_ORDER_UNITS || unit == GSB_ORDER_UNIT_MP_RELAXED || smid >= GSB_SM_MAX || index >= GSB_ORDER_OBS_MAX)
+    return GSB_ERR_INVALID_ARGUMENT;
+  Device *d = device_at(idx);
+  if (!d) return G.inited ? GSB_ERR_NO_DEVICE : GSB_ERR_NOT_INITIALIZED;
+  std::lock_guard<std::mutex> lk(d->smu);
+  Device::OrderInject &h = d->order.hooks.inject[unit];
+  h.armed = true;
+  h.smid = smid;
+  h.index = index;
+  return GSB_OK;
+}
+
+int gsb_test_order_skip(uint32_t idx, uint32_t smid) {
+  std::shared_lock<std::shared_mutex> api_lk(G.api_mu);
+  if (smid >= GSB_SM_MAX) return GSB_ERR_INVALID_ARGUMENT;
+  Device *d = device_at(idx);
+  if (!d) return G.inited ? GSB_ERR_NO_DEVICE : GSB_ERR_NOT_INITIALIZED;
+  std::lock_guard<std::mutex> lk(d->smu);
+  d->order.hooks.skip_armed = true;
+  d->order.hooks.skip_smid = smid;
   return GSB_OK;
 }
 

@@ -257,6 +257,44 @@ int gsb_l1_occupancy(uint32_t unit, int *ctas);
 /* Load the L1 check's kernels into the CURRENT context and ask for the largest L1 (carveout 0) for its buffer units. */
 int gsb_l1_kernel_preload(void);
 
+/* What one memory-ordering check launch (order_check_sm90a.cu) leaves in device memory; the host zeroes it before every
+ * launch. Its leading fields are the SM check's, so fold_log serves it. */
+struct gsb_order_log {
+  unsigned int covered[GSB_SM_MAX / 32]; /* bit %smid: a CTA of the launch ran there */
+  unsigned int faulty[GSB_SM_MAX / 32];  /* bit %smid: a consumer there recorded a bad outcome */
+  unsigned long long words;              /* u64 words read and checked */
+  unsigned long long mismatch_words;     /* observations and final reads classed CORRUPT, FORBIDDEN or LOST */
+  unsigned long long mismatch_bits;
+  unsigned int count;                    /* records claimed (may pass GSB_ORDER_RECORDS) */
+  unsigned int barrier;                  /* the grid barriers' arrival counter */
+  unsigned long long corrupt, forbidden, lost, timeout, overlap, weak;
+  gsb_order_record rec[GSB_ORDER_RECORDS];
+};
+
+struct gsb_order_args {
+  gsb_order_log *log;
+  unsigned long long *locs;  /* sm_count blocks of GSB_ORDER_LOC_WORDS u64 */
+  uint4 *scratch;            /* sm_count stress regions of GSB_ORDER_SCRATCH_WORDS */
+  unsigned long long *obs;   /* [rank][observation][GSB_ORDER_OBS_WORDS]: SB and IRIW reads, classified after the barrier */
+  uint32_t *smids;           /* [rank]: %smid, published before the first barrier */
+  uint32_t seed;             /* the seed the words are stored under */
+  uint32_t seed_expect;      /* the seed the kernel checks hashes against */
+  uint32_t unit;             /* GSB_ORDER_UNIT_* */
+  uint32_t distance;         /* d */
+  uint32_t dist_index;       /* 0..GSB_ORDER_DISTANCES-1, for the records */
+  uint32_t observations;     /* iterations per CTA */
+  uint32_t inject_smid;      /* test hook: the consumer on this SM forges observation inject_index; GSB_SM_MAX: none */
+  uint32_t inject_index;
+  uint32_t skip_smid;        /* test hook: the CTA on this SM stores nothing; GSB_SM_MAX: none */
+  uint32_t smem_bytes;       /* dynamic shared memory of every CTA */
+};
+
+/* Enqueue one cooperative memory-ordering launch of `grid` CTAs on `stream`. Returns cudaError_t as int
+ * (cudaErrorCooperativeLaunchTooLarge: the CTAs could not all be co-resident). */
+int gsb_order_kernel_launch(uint32_t grid, const gsb_order_args *a, cudaStream_t stream);
+/* Load its kernel into the CURRENT context and let it take `smem_bytes` of dynamic shared memory. */
+int gsb_order_kernel_preload(int smem_bytes);
+
 /* What one SM-stress slice (sm_stress_sm90a.cu) leaves in device memory; the host zeroes it before every slice. */
 struct gsb_stress_log {
   unsigned int covered[GSB_SM_MAX / 32];

@@ -974,6 +974,73 @@ test_l1_skip.__test__ = False
 test_l1_table.__test__ = False
 
 
+def order_probe(idx: int, *, seed: int = 0, seed_expect: int = 0, units: int = 0, observations: int = 0,
+                raise_on_error: bool = True) -> "_abi.OrderResult":
+    """Memory-ordering probe of device `idx`: each unit (`units`: a mask of 1 << GSB_ORDER_UNIT_*, 0 = all) at three
+    distances, `observations` per CTA and launch (0 = 1024), every word's hash checked against `seed_expect` (0 =
+    `seed`; `seed` 0 = fresh). Outcomes are a result, not an error; with raise_on_error=False a failed launch is too
+    (``status`` < 0)."""
+    cfg = _abi.OrderCfg(seed, seed_expect, units, observations)
+    r = _abi.OrderResult()
+    rc = lib.gsb_order_probe(idx, C.byref(cfg), C.byref(r))
+    if raise_on_error:
+        check(rc, f"gsb_order_probe({idx})")
+    return r
+
+
+def order_stats(idx: int) -> "_abi.OrderStats":
+    """Memory-ordering probes of device `idx` since health_start: count, faults, skipped, incomplete, the last result."""
+    st = _abi.OrderStats()
+    check(lib.gsb_order_stats_get(idx, C.byref(st)), f"gsb_order_stats_get({idx})")
+    return st
+
+
+def order_pairing(unit: int, n: int, d: int, rank: int) -> list:
+    """gsb_order_pairing: the ranks CTA `rank` of `n` reads in `unit` at distance `d` ([] for a bad argument)."""
+    out = (C.c_uint32 * 3)()
+    k = lib.gsb_order_pairing(unit, n, d, rank, out)
+    return list(out[:k])
+
+
+def order_classify(unit: int, seed: int, keys, words, iteration: int = 0) -> int:
+    """gsb_order_classify: the GSB_ORDER_CLS_* class of one observation."""
+    k = (C.c_uint32 * _abi.GSB_ORDER_WORDS)(*list(keys)[:_abi.GSB_ORDER_WORDS])
+    w = (C.c_uint64 * _abi.GSB_ORDER_WORDS)(*list(words)[:_abi.GSB_ORDER_WORDS])
+    return int(lib.gsb_order_classify(unit, seed, k, w, iteration))
+
+
+def order_conditions(r: "_abi.OrderResult") -> int:
+    """GSB_ORDER_* bits a memory-ordering probe result raises."""
+    return lib.gsb_order_conditions(C.byref(r))
+
+
+def order_text(r: "_abi.OrderResult", uuid: str) -> str:
+    """The one log line both daemons print for a memory-ordering probe result."""
+    need = lib.gsb_order_text(C.byref(r), uuid.encode(), None, 0)
+    check(int(need), "gsb_order_text(size)")
+    buf = C.create_string_buffer(int(need))
+    n = lib.gsb_order_text(C.byref(r), uuid.encode(), buf, int(need))
+    check(int(n), "gsb_order_text")
+    return buf.raw[: int(n)].decode()
+
+
+def test_order_inject(idx: int, smid: int, unit: int, index: int) -> None:
+    """Test hook: on the next memory-ordering probe of `idx`, the consumer on SM `smid` reports observation `index` of
+    `unit`'s first launch as a forbidden outcome with valid hashes; once. The next probe takes it whatever its
+    observations; an index at or past them injects nothing."""
+    check(lib.gsb_test_order_inject(idx, smid, unit, index), f"gsb_test_order_inject({idx})")
+
+
+def test_order_skip(idx: int, smid: int) -> None:
+    """Test hook: in the next memory-ordering probe of `idx`, the producer on SM `smid` stores nothing in the first
+    MP_RELACQ launch; once."""
+    check(lib.gsb_test_order_skip(idx, smid), f"gsb_test_order_skip({idx})")
+
+
+test_order_inject.__test__ = False
+test_order_skip.__test__ = False
+
+
 def fault_classify(offset: int, expected, observed) -> FaultRecord:
     """gsb_fault_classify of one word: cls, alias_bit, seed_key and flipped_bits filled in."""
     rec = FaultRecord(offset, (C.c_uint32 * 4)(*expected), (C.c_uint32 * 4)(*observed))

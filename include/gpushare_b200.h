@@ -46,7 +46,8 @@ extern "C" {
                               by gsb_atomic_probe; tensor-core format health (gsb_tensor_*, GSB_EVENT_TENSOR)
                               likewise, found by gsb_tensor_probe; SM special-function health (gsb_sfu_*,
                               GSB_EVENT_SFU) likewise, found by gsb_sfu_probe; L1 and constant-cache health
-                              (gsb_l1_*, GSB_EVENT_L1) likewise, found by gsb_l1_probe */
+                              (gsb_l1_*, GSB_EVENT_L1) likewise, found by gsb_l1_probe; memory-ordering health
+                              (gsb_order_*, GSB_EVENT_ORDER) likewise, found by gsb_order_probe */
 
 /* = NVML_DEVICE_UUID_BUFFER_SIZE (vendor/.../nvml/nvml.h:1567), used by bindings.go:20 szUUID */
 #define GSB_UUID_BUFFER_SIZE 80
@@ -166,9 +167,14 @@ enum {
                                             link, copy, SM, SM-to-SM, L2 atomic and tensor-core format probes when
                                             they are due), and raises GSB_EVENT_SFU; 0 = off (default): no buffer, no
                                             launch */
-  GSB_OPT_L1_PROBE_EVERY_CYCLES = 15      /* N > 0: each prober thread runs gsb_l1_probe after its first cycle of a
-                                            health session and after every Nth cycle, outside gsb_cycle (after every
-                                            other periodic probe that is due), and raises GSB_EVENT_L1; 0 = off
+  GSB_OPT_L1_PROBE_EVERY_CYCLES = 15,     /* N > 0: each prober thread runs gsb_l1_probe after its first cycle of a
+                                            health session and after every Nth cycle, outside gsb_cycle (after the
+                                            link, copy, SM, SM-to-SM, L2 atomic, tensor-core format and SFU probes
+                                            when they are due), and raises GSB_EVENT_L1; 0 = off (default): no
+                                            buffer, no launch */
+  GSB_OPT_ORDER_PROBE_EVERY_CYCLES = 16   /* N > 0: each prober thread runs gsb_order_probe after its first cycle of
+                                            a health session and after every Nth cycle, outside gsb_cycle (after every
+                                            other periodic probe that is due), and raises GSB_EVENT_ORDER; 0 = off
                                             (default): no buffer, no launch */
 };
 enum {
@@ -334,8 +340,10 @@ enum {
                                   GSB_TENSOR_* bit */
   GSB_EVENT_SFU = 0x20000,     /* GSB_OPT_SFU_PROBE_EVERY_CYCLES: an SM special-function condition; edata = one
                                   GSB_SFU_* bit */
-  GSB_EVENT_L1 = 0x40000       /* GSB_OPT_L1_PROBE_EVERY_CYCLES: an L1 or constant-cache condition; edata = one
+  GSB_EVENT_L1 = 0x40000,      /* GSB_OPT_L1_PROBE_EVERY_CYCLES: an L1 or constant-cache condition; edata = one
                                   GSB_L1_* bit */
+  GSB_EVENT_ORDER = 0x80000    /* GSB_OPT_ORDER_PROBE_EVERY_CYCLES: a memory-ordering condition; edata = one
+                                  GSB_ORDER_* bit */
 };
 enum { GSB_PROBE_FAULT_MISMATCH = 1, GSB_PROBE_FAULT_LAUNCH = 2, GSB_PROBE_RECOVERED = 3,
        GSB_PROBE_FAULT_WEDGED = 4 /* the launch outlived the completion watchdog */ };
@@ -1781,6 +1789,168 @@ int gsb_test_l1_skip(uint32_t idx, uint32_t smid);
  * device's sm_count CTAs is refused once the device is known. */
 int gsb_test_l1_table(uint32_t idx, uint32_t unit, const uint32_t *table, size_t n, const uint32_t *expected,
                       size_t n_expected, uint32_t region_words);
+
+/* ---- Memory-ordering health (not in the reference; opt-in: GSB_OPT_ORDER_PROBE_EVERY_CYCLES) ------------------- */
+
+/*
+ * Litmus tests of the PTX memory model at .gpu scope between SMs, through L2. Each unit runs at three distances d
+ * (gsb_order_distance): one cooperative launch of sm_count CTAs of GSB_ORDER_THREADS, one per SM (the opt-in maximum
+ * of dynamic shared memory), all co-resident. CTA rank r pairs with (r + d) mod n; thread 0 plays the litmus role and
+ * warps 1-7 load and store (.cg) the CTA's own 64 KiB scratch region to perturb timing (not judged). Every shared
+ * location is one aligned u64 (single-copy atomic): high 32 bits the iteration i, low 32 bits gsb_mix32(seed ^ key ^
+ * i), key the location's gsb_order_key; a word whose low half is not that hash is CORRUPT. Every CTA writes its own
+ * locations with i = 1..observations and observes its partners' once per iteration:
+ *
+ *   MP_RELACQ   4 data st.relaxed.gpu, st.release.gpu flag | ld.acquire.gpu flag, 4 data ld.relaxed.gpu
+ *   MP_FENCE    relaxed data, fence.acq_rel.gpu, relaxed flag | relaxed flag, fence.acq_rel.gpu, relaxed data
+ *               forbidden (both MP units): a data iteration below the flag's
+ *   SB_SC       st x_r = i; fence.sc.gpu; ld x_(r+d); ld x_(r-d); fence.sc.gpu. Instance r is (r, r + d): forbidden in
+ *               iteration i, both reads of the other's word < i, or both > i
+ *   IRIW_SC     instance r: writers r (x) and r + e (y), readers r + 2e (a = ld x; fence.sc; b = ld y) and r + 3e
+ *               (c = ld y; fence.sc; d = ld x), e = gsb_order_iriw_distance: forbidden for the k-th observations of
+ *               both readers, a > d and c > b
+ *   CORR        st.relaxed x = i | two ld.relaxed of x per observation: forbidden, a read older than the one before it
+ *               (in the observation or the previous one)
+ *   MP_RELAXED  relaxed data, relaxed flag, no fence, both sides: a data iteration below the flag's is counted (weak),
+ *               never a condition; it shows whether the test can see reordering at all
+ *
+ * After the last observation every CTA meets at a grid barrier (release/acquire on a counter, bounded by
+ * GSB_ORDER_WAIT_NS plus GSB_ORDER_WAIT_NS_PER_OBS per observation of %globaltimer, since the slowest CTA's loop may
+ * trail the fastest's; one that runs out is TIMEOUT, as is the first barrier, before the loop, after GSB_ORDER_WAIT_NS);
+ * then every consumer reads each location it
+ * observed once more and must see iteration `observations` (older: LOST). Each CTA classifies its own observations
+ * (gsb_order_classify) and records CORRUPT, FORBIDDEN and LOST ones; "overlap" counts observations that saw a partner
+ * mid-stream (the race window was hit). Overlap and weak counts are logged, never judged.
+ */
+enum {
+  GSB_ORDER_UNIT_MP_RELACQ = 0,
+  GSB_ORDER_UNIT_MP_FENCE = 1,
+  GSB_ORDER_UNIT_SB_SC = 2,
+  GSB_ORDER_UNIT_IRIW_SC = 3,
+  GSB_ORDER_UNIT_CORR = 4,
+  GSB_ORDER_UNIT_MP_RELAXED = 5
+};
+#define GSB_ORDER_UNITS 6
+#define GSB_ORDER_DISTANCES 3          /* launches per unit: d = 1, n / 2, 1 + seed mod (n - 1) */
+#define GSB_ORDER_THREADS 256
+#define GSB_ORDER_OBS_DEFAULT 1024
+#define GSB_ORDER_OBS_MAX 65536
+#define GSB_ORDER_WORDS 5              /* words of one observation (MP: the flag, then 4 data) */
+#define GSB_ORDER_RECORDS 64
+#define GSB_ORDER_WAIT_NS 100000000ull /* a grid barrier's %globaltimer bound */
+#define GSB_ORDER_WAIT_NS_PER_OBS 5000ull /* the second barrier's bound grows by this per observation */
+/* outcome classes of one observation (gsb_order_classify) */
+enum {
+  GSB_ORDER_CLS_ALLOWED = 0,   /* an outcome the model allows, no partner mid-stream */
+  GSB_ORDER_CLS_OVERLAP = 1,   /* allowed, and a partner was seen mid-stream */
+  GSB_ORDER_CLS_WEAK = 2,      /* MP_RELAXED: a data iteration below the flag's (allowed there) */
+  GSB_ORDER_CLS_FORBIDDEN = 3, /* an outcome the model forbids */
+  GSB_ORDER_CLS_CORRUPT = 4,   /* a word whose low half is not the hash of its high half */
+  GSB_ORDER_CLS_LOST = 5       /* a final read older than the writer's last iteration */
+};
+
+typedef struct gsb_order_cfg {
+  uint32_t seed;         /* the words' seed; 0 = fresh per probe */
+  uint32_t seed_expect;  /* seed the kernels check hashes against; 0 = seed */
+  uint32_t units;        /* mask of 1 << GSB_ORDER_UNIT_*; 0 = all */
+  uint32_t observations; /* per CTA and launch, 1..GSB_ORDER_OBS_MAX; 0 = GSB_ORDER_OBS_DEFAULT */
+} gsb_order_cfg;
+
+/* One CORRUPT, FORBIDDEN or LOST observation. producer: the %smid of the CTAs whose stores or reads its words show,
+ * GSB_SM_MAX where there are fewer: MP and CORR the producer r + d; SB the partner r + d (writer of the x_(r+d) this CTA
+ * read) and this CTA r itself (writer of the x_r the partner read); IRIW the writers of x and y and the other reader
+ * (gsb_order_pairing's order); LOST the writer of the location read. words: as gsb_order_classify takes them (LOST:
+ * the final word). */
+typedef struct gsb_order_record {
+  uint32_t unit, distance;  /* distance: 0..GSB_ORDER_DISTANCES-1 */
+  uint32_t cls;             /* GSB_ORDER_CLS_* */
+  uint32_t smid;            /* the consumer's */
+  uint32_t producer[3];
+  uint32_t index;           /* observation (iteration - 1); LOST: the location's slot in gsb_order_pairing's order */
+  uint64_t words[GSB_ORDER_WORDS];
+} gsb_order_record;
+
+typedef struct gsb_order_unit_result {
+  int32_t status;           /* GSB_OK, or the first failed launch's gsb_status (GSB_ERR_TIMEOUT: outlived the watchdog) */
+  uint32_t launches;        /* launches that ran (0 = the unit did not run) */
+  uint32_t refused;         /* launches refused for co-residency: skipped, counted, not a condition */
+  uint32_t sms_covered;     /* SMs covered, as producer and consumer, by every launch that ran */
+  uint64_t words_checked;   /* u64 words read and checked, over every CTA of every launch */
+  uint64_t mismatch_words;  /* observations and final reads classed CORRUPT, FORBIDDEN or LOST */
+  uint64_t mismatch_bits;   /* bits of CORRUPT words' low halves that differ from the hash */
+  uint64_t corrupt, forbidden, lost, timeout;
+  uint64_t overlap;         /* observations that saw a partner mid-stream (logged only) */
+  uint64_t weak;            /* MP_RELAXED: weak outcomes (logged only) */
+  uint64_t kernel_ns;       /* CUDA-event time of its launches */
+} gsb_order_unit_result;
+
+typedef struct gsb_order_result {
+  int32_t status;           /* GSB_OK iff every unit asked for ran or was refused (outcomes are a result) */
+  uint32_t sm_count;        /* the device's multiProcessorCount = the grid of every launch */
+  uint32_t seed, seed_expect, units, observations;
+  uint32_t distance[GSB_ORDER_DISTANCES];
+  uint32_t sms_covered;     /* SMs covered by every unit that ran */
+  uint32_t n_records;       /* records filled (the first GSB_ORDER_RECORDS) */
+  uint32_t covered[GSB_SM_MAX / 32];  /* their bitmap, bit smid */
+  uint32_t faulty[GSB_SM_MAX / 32];   /* consumers' SMs with a CORRUPT, FORBIDDEN or LOST observation */
+  gsb_order_unit_result unit[GSB_ORDER_UNITS];
+  gsb_order_record records[GSB_ORDER_RECORDS];
+  uint64_t wall_ns;         /* host time of the whole call */
+} gsb_order_result;
+
+/* Conditions (gsb_order_conditions), from the units that ran only. Overlap and weak counts and refused launches are
+ * never conditions. */
+enum {
+  GSB_ORDER_CORRUPT = 1u,   /* a word read back is not a word any writer stored */
+  GSB_ORDER_FORBIDDEN = 2u, /* an outcome the PTX memory model forbids at .gpu scope */
+  GSB_ORDER_LOST = 4u,      /* a final read after the grid barrier older than the writer's last store */
+  GSB_ORDER_TIMEOUT = 8u,   /* a grid barrier ran out: an SM stalled or a store never became visible */
+  GSB_ORDER_FAILED = 16u    /* a launch failed or outlived the watchdog */
+};
+
+/* Memory-ordering probes of one device since gsb_health_start (counters restart with it; gsb_order_probe calls count
+ * too). */
+typedef struct gsb_order_stats {
+  uint64_t probes;     /* probes run */
+  uint64_t faults;     /* of which raised at least one GSB_ORDER_* condition */
+  uint64_t skipped;    /* probes that ran no launch (buffer not allocatable, every launch refused): no condition */
+  uint64_t incomplete; /* probes in which some unit covered fewer than sm_count SMs or had a launch refused */
+  gsb_order_result last;
+} gsb_order_stats;
+
+/* Holds the device while it runs; each launch under the completion watchdog. One transient buffer of sm_count x
+ * (80 KiB + 32 B per observation) plus the launch log, taken only while GSB_OPT_TRANSIENT_KEEP_FREE_BYTES stays free; a
+ * probe that cannot take it returns GSB_ERR_OUT_OF_MEMORY and counts as skipped. */
+int gsb_order_probe(uint32_t idx, const gsb_order_cfg *cfg, gsb_order_result *out);
+int gsb_order_stats_get(uint32_t idx, gsb_order_stats *out);
+/* Pure: the distance of launch k (0..GSB_ORDER_DISTANCES-1) on n CTAs under seed; 0 when n < 2 or k is out of range. */
+uint32_t gsb_order_distance(uint32_t k, uint32_t n, uint32_t seed);
+/* Pure: IRIW's step e for distance d on n CTAs: the first of d, d + 1, ... (mod n, skipping 0) with e, 2e and 3e all
+ * nonzero mod n; 0 when n < 4. */
+uint32_t gsb_order_iriw_distance(uint32_t n, uint32_t d);
+/* Pure: the ranks CTA `rank` of n reads in `unit` at distance d, in the order its observation's words take them
+ * (MP: the producer; SB: r + d, then r - d whose read of x_r is the partner's half; IRIW: x, y, and the other reader
+ * r + e of the instance r - 2e it classifies; CORR: the writer). Returns how many (0: a bad argument). */
+int gsb_order_pairing(uint32_t unit, uint32_t n, uint32_t d, uint32_t rank, uint32_t ranks[3]);
+/* Pure: the class of one observation. words as the consumer holds them (MP: flag, data 0-3; SB: its read of x_(r+d),
+ * the partner's read of x_r; IRIW: a, b, c, d; CORR: the previous read, then the observation's two), keys each word's
+ * location key, iteration the SB iteration (1..), seed the seed the hashes are checked against. GSB_ORDER_CLS_CORRUPT
+ * for an unknown unit. */
+uint32_t gsb_order_classify(uint32_t unit, uint32_t seed, const uint32_t keys[GSB_ORDER_WORDS],
+                            const uint64_t words[GSB_ORDER_WORDS], uint32_t iteration);
+/* Pure: GSB_ORDER_* bits that hold for a result (see above). */
+uint32_t gsb_order_conditions(const gsb_order_result *r);
+/* Pure: the one-line text both daemons log for a result. uuid may be NULL. Returns like gsb_sm_text. */
+int64_t gsb_order_text(const gsb_order_result *r, const char *uuid, char *buf, size_t cap);
+/* test hook: on the next gsb_order_probe of device idx, the consumer on SM `smid` reports observation `index` of
+ * `unit`'s first launch as a forbidden outcome with valid hashes. Refused before any device is touched: unit out of
+ * range or MP_RELAXED (which forbids nothing), smid >= GSB_SM_MAX, index >= GSB_ORDER_OBS_MAX. The next probe takes
+ * the hook whatever its observations; an index at or past them (known only then) injects nothing. */
+int gsb_test_order_inject(uint32_t idx, uint32_t smid, uint32_t unit, uint32_t index);
+/* test hook: in the next gsb_order_probe of device idx, the producer on SM `smid` writes nothing in the first
+ * MP_RELACQ launch, so its consumer reads every location LOST. Refused before any device is touched when smid >=
+ * GSB_SM_MAX. */
+int gsb_test_order_skip(uint32_t idx, uint32_t smid);
 
 /* ---- Allocate (a12, a13): wire bytes in, wire bytes out ---------------------------------- */
 

@@ -99,6 +99,7 @@ const (
 	gsbEventTensor    = uint64(C.GSB_EVENT_TENSOR)    // opt-in tensor-core format health: Edata = one of the gsbTensor* conditions below
 	gsbEventSFU       = uint64(C.GSB_EVENT_SFU)       // opt-in SM special-function health: Edata = one of the gsbSFU* conditions below
 	gsbEventL1        = uint64(C.GSB_EVENT_L1)        // opt-in L1 and constant-cache health: Edata = one of the gsbL1* conditions below
+	gsbEventOrder     = uint64(C.GSB_EVENT_ORDER)     // opt-in memory-ordering health: Edata = one of the gsbOrder* conditions below
 )
 
 const (
@@ -142,6 +143,14 @@ const (
 const (
 	gsbL1Corrupt = uint64(C.GSB_L1_CORRUPT) // a word read through L1, texture, constant bank or kernel parameters is wrong on some SM
 	gsbL1Failed  = uint64(C.GSB_L1_FAILED)  // an L1-check launch failed or outlived the watchdog
+)
+
+const (
+	gsbOrderCorrupt   = uint64(C.GSB_ORDER_CORRUPT)   // a word read back between SMs is not one any writer stored
+	gsbOrderForbidden = uint64(C.GSB_ORDER_FORBIDDEN) // an outcome the PTX memory model forbids at .gpu scope
+	gsbOrderLost      = uint64(C.GSB_ORDER_LOST)      // a store not visible after the grid barrier
+	gsbOrderTimeout   = uint64(C.GSB_ORDER_TIMEOUT)   // a grid barrier ran out: an SM stalled or a store never became visible
+	gsbOrderFailed    = uint64(C.GSB_ORDER_FAILED)    // a memory-ordering launch failed or outlived the watchdog
 )
 
 const (
@@ -609,6 +618,34 @@ func gsbL1Line(idx uint, uuid string) string {
 	}
 	buf := make([]byte, int(need))
 	n := C.gsb_l1_text(&st.last, cu, (*C.char)(unsafe.Pointer(&buf[0])), C.size_t(len(buf)))
+	if n < 0 {
+		return ""
+	}
+	return string(buf[:int(n)])
+}
+
+// gsbEnableOrderHealth turns on memory-ordering health: each prober runs gsb_order_probe after its first cycle of a
+// session and after every `every`-th cycle. Call it before gsbHealthStart.
+func gsbEnableOrderHealth(every uint64) error {
+	return gsbErr(C.gsb_set_option(C.GSB_OPT_ORDER_PROBE_EVERY_CYCLES, C.uint64_t(every)))
+}
+
+// gsbOrderLine is the one log line of GPU idx's most recent memory-ordering probe ("not run" when there is none):
+// what a plugin logs before marking a GPU unhealthy on a GSB_EVENT_ORDER event.
+func gsbOrderLine(idx uint, uuid string) string {
+	st := (*C.gsb_order_stats)(C.calloc(1, C.size_t(unsafe.Sizeof(C.gsb_order_stats{}))))
+	defer C.free(unsafe.Pointer(st))
+	if C.gsb_order_stats_get(C.uint32_t(idx), st) != C.GSB_OK {
+		*st = C.gsb_order_stats{}
+	}
+	cu := C.CString(uuid)
+	defer C.free(unsafe.Pointer(cu))
+	need := C.gsb_order_text(&st.last, cu, nil, 0)
+	if need <= 0 {
+		return ""
+	}
+	buf := make([]byte, int(need))
+	n := C.gsb_order_text(&st.last, cu, (*C.char)(unsafe.Pointer(&buf[0])), C.size_t(len(buf)))
 	if n < 0 {
 		return ""
 	}
