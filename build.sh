@@ -14,6 +14,7 @@ $NVCC $FLAGS -Xptxas -v -c $SRC/sm_check_sm90a.cu -o build/sm_check_sm90a.o 2> b
 $NVCC $FLAGS -Xptxas -v -c $SRC/mma_operands_sm90a.cu -o build/mma_operands_sm90a.o 2> build/ptxas_mma_operands.log || { cat build/ptxas_mma_operands.log; exit 1; }
 $NVCC $FLAGS -Xptxas -v -c $SRC/sm_stress_sm90a.cu -o build/sm_stress_sm90a.o 2> build/ptxas_sm_stress.log || { cat build/ptxas_sm_stress.log; exit 1; }
 $NVCC $FLAGS -Xptxas -v -c $SRC/cluster_check_sm90a.cu -o build/cluster_check_sm90a.o 2> build/ptxas_cluster_check.log || { cat build/ptxas_cluster_check.log; exit 1; }
+$NVCC $FLAGS -Xptxas -v -c $SRC/cluster_script_sm90a.cu -o build/cluster_script_sm90a.o 2> build/ptxas_cluster_script.log || { cat build/ptxas_cluster_script.log; exit 1; }
 $NVCC $FLAGS -Xptxas -v -c $SRC/atomic_check_sm90a.cu -o build/atomic_check_sm90a.o 2> build/ptxas_atomic_check.log || { cat build/ptxas_atomic_check.log; exit 1; }
 $NVCC $FLAGS -Xptxas -v -c $SRC/atomic_values_sm90a.cu -o build/atomic_values_sm90a.o 2> build/ptxas_atomic_values.log || { cat build/ptxas_atomic_values.log; exit 1; }
 $NVCC $FLAGS -Xptxas -v -c $SRC/tensor_check_sm90a.cu -o build/tensor_check_sm90a.o 2> build/ptxas_tensor_check.log || { cat build/ptxas_tensor_check.log; exit 1; }
@@ -30,6 +31,9 @@ $NVCC -shared -gencode arch=compute_90a,code=sm_90a -cudart static -o $PKG/libgp
 # the memory-ordering check's kernel is a module of its own too: the kernel set of libgpushare_b200.so and of the L1
 # module is pinned with its recorded SASS (tests/golden/shipped_kernels_sass.json)
 $NVCC -shared -gencode arch=compute_90a,code=sm_90a -cudart static -o $PKG/libgpushare_b200_order.so build/order_check_sm90a.o
+# the SM-to-SM check's test-only twins likewise: the shipped cluster_check kernels stay in the main library, whose
+# recorded kernel set the twins leave as it is; the twins are pinned in tests/golden/cluster_script_sass.json
+$NVCC -shared -gencode arch=compute_90a,code=sm_90a -cudart static -o $PKG/libgpushare_b200_cluster_script.so build/cluster_script_sm90a.o
 $NVCC $FLAGS -c $SRC/gsb_device.cu -o build/gsb_device.o
 g++ -O2 -std=c++17 -fPIC -Wall -c $SRC/gsb_wire.cc -o build/gsb_wire.o
 g++ -O2 -std=c++17 -fPIC -Wall -c $SRC/gsb_fault.cc -o build/gsb_fault.o
@@ -45,7 +49,7 @@ g++ -O2 -std=c++17 -fPIC -Wall -c $SRC/gsb_tensor.cc -o build/gsb_tensor.o
 g++ -O2 -std=c++17 -fPIC -Wall -c $SRC/gsb_sfu.cc -o build/gsb_sfu.o
 g++ -O2 -std=c++17 -fPIC -Wall -c $SRC/gsb_l1.cc -o build/gsb_l1.o
 g++ -O2 -std=c++17 -fPIC -Wall -c $SRC/gsb_order.cc -o build/gsb_order.o
-$NVCC -shared -gencode arch=compute_90a,code=sm_90a -cudart static -o $OUT build/hbm_probe_sm90a.o build/sm_check_sm90a.o build/mma_operands_sm90a.o build/sm_stress_sm90a.o build/cluster_check_sm90a.o build/atomic_check_sm90a.o build/atomic_values_sm90a.o build/tensor_check_sm90a.o build/tensor_operands_sm90a.o build/sfu_check_sm90a.o build/sfu_operands_sm90a.o build/gsb_device.o build/gsb_wire.o build/gsb_fault.o build/gsb_ecc.o build/gsb_memtest.o build/gsb_link.o build/gsb_copy.o build/gsb_sm.o build/gsb_stress.o build/gsb_cluster.o build/gsb_atomic.o build/gsb_tensor.o build/gsb_sfu.o build/gsb_l1.o build/gsb_order.o -L$PKG -lgpushare_b200_l1 -lgpushare_b200_order -Xlinker -rpath,'$ORIGIN' -ldl -lpthread -lrt
+$NVCC -shared -gencode arch=compute_90a,code=sm_90a -cudart static -o $OUT build/hbm_probe_sm90a.o build/sm_check_sm90a.o build/mma_operands_sm90a.o build/sm_stress_sm90a.o build/cluster_check_sm90a.o build/atomic_check_sm90a.o build/atomic_values_sm90a.o build/tensor_check_sm90a.o build/tensor_operands_sm90a.o build/sfu_check_sm90a.o build/sfu_operands_sm90a.o build/gsb_device.o build/gsb_wire.o build/gsb_fault.o build/gsb_ecc.o build/gsb_memtest.o build/gsb_link.o build/gsb_copy.o build/gsb_sm.o build/gsb_stress.o build/gsb_cluster.o build/gsb_atomic.o build/gsb_tensor.o build/gsb_sfu.o build/gsb_l1.o build/gsb_order.o -L$PKG -lgpushare_b200_l1 -lgpushare_b200_order -lgpushare_b200_cluster_script -Xlinker -rpath,'$ORIGIN' -ldl -lpthread -lrt
 echo "built $OUT"
 # native daemon (C++ host side: HTTP/2 + HPACK gRPC front end, kube client, manager loop) + its h2 self-test
 g++ -O2 -std=c++17 -Wall -pthread -o $PKG/gsbd $SRC/daemon/gsbd.cc -L$PKG -lgpushare_b200 -lssl -lcrypto -ldl -Wl,-rpath,'$ORIGIN'

@@ -16,6 +16,8 @@ LIB_PATH = os.path.join(_HERE, "libgpushare_b200.so")
 L1_LIB_PATH = os.path.join(_HERE, "libgpushare_b200_l1.so")
 # the memory-ordering check's kernel, likewise a module of its own that LIB_PATH loads
 ORDER_LIB_PATH = os.path.join(_HERE, "libgpushare_b200_order.so")
+# the SM-to-SM check's test-only twins (gsb_test_cluster_script), likewise a module of their own that LIB_PATH loads
+CLUSTER_SCRIPT_LIB_PATH = os.path.join(_HERE, "libgpushare_b200_cluster_script.so")
 
 GSB_UUID_BUFFER_SIZE = 80
 GSB_BUSID_BUFFER_SIZE = 32
@@ -63,6 +65,7 @@ CLUSTER_PATH_NAMES = ["dsmem_st", "dsmem_ld", "st_async", "bulk_s2s", "multicast
 GSB_CLUSTER_PATHS, GSB_CLUSTER_SIZES, GSB_CLUSTER_MAX_N, GSB_CLUSTER_RECORDS, GSB_CLUSTER_MAX_LAUNCHES = 5, 4, 16, 64, 3
 GSB_CLUSTER_SM_MAX, GSB_CLUSTER_WAIT_NS, GSB_CLUSTER_EVERY_RANK, GSB_CLUSTER_HEADER_BYTES = 256, 100000000, 0xFF, 1024
 GSB_CLUSTER_HOOK_INDEX_MAX = 14464
+GSB_CLUSTER_UNROUTED = 0xFF
 GSB_CLUSTER_CORRUPT, GSB_CLUSTER_FAILED = 1, 2
 CLUSTER_CONDITION_NAMES = {1: "wrong word across the SM-to-SM network", 2: "SM-to-SM probe failed"}
 GSB_CLUSTER_CLASS_ZERO, GSB_CLUSTER_CLASS_STALE, GSB_CLUSTER_CLASS_MISROUTED, GSB_CLUSTER_CLASS_BITS = 1, 2, 3, 4
@@ -180,7 +183,7 @@ SYMBOLS = [
     "gsb_test_sm_operands",
     "gsb_sm_stress", "gsb_stress_fold", "gsb_stress_conditions", "gsb_stress_text", "gsb_test_stress_corrupt",
     "gsb_cluster_probe", "gsb_cluster_stats_get", "gsb_cluster_conditions", "gsb_cluster_classify", "gsb_cluster_text",
-    "gsb_test_cluster_corrupt", "gsb_test_cluster_skip",
+    "gsb_test_cluster_corrupt", "gsb_test_cluster_skip", "gsb_test_cluster_script",
     "gsb_atomic_probe", "gsb_atomic_stats_get", "gsb_atomic_expected", "gsb_atomic_conditions", "gsb_atomic_text",
     "gsb_test_atomic_corrupt", "gsb_test_atomic_skip", "gsb_test_atomic_values",
     "gsb_tensor_probe", "gsb_tensor_stats_get", "gsb_tensor_expected", "gsb_tensor_conditions", "gsb_tensor_text",
@@ -1159,6 +1162,7 @@ def _load() -> C.CDLL:
         "gsb_cluster_text": (C.c_int64, [C.POINTER(ClusterResult), C.c_char_p, C.c_char_p, C.c_size_t]),
         "gsb_test_cluster_corrupt": (C.c_int, [C.c_uint32, C.c_uint32, C.c_uint32, C.c_uint32, C.c_uint64]),
         "gsb_test_cluster_skip": (C.c_int, [C.c_uint32, C.c_uint32, C.c_uint32]),
+        "gsb_test_cluster_script": (C.c_int, [C.c_uint32, C.c_uint32, C.c_uint32, C.c_uint32, u8p]),
         "gsb_atomic_probe": (C.c_int, [C.c_uint32, C.POINTER(AtomicCfg), C.POINTER(AtomicResult)]),
         "gsb_atomic_stats_get": (C.c_int, [C.c_uint32, C.POINTER(AtomicStats)]),
         "gsb_atomic_expected": (C.c_int64, [C.c_uint32, C.c_uint32, C.c_uint32, C.c_void_p, C.c_size_t]),

@@ -3,12 +3,8 @@
  * thread-block cluster over the SM-to-SM network, one kernel per path. Host code lives in gsb_device.cu (the probe) and
  * gsb_cluster.cc (policy, classification, text); the geometry and the words are defined in gsb_cluster.h.
  *
- * Every CTA asks for the device's opt-in maximum of dynamic shared memory, so each CTA of a cluster runs on its own SM.
- * It writes its %smid and %cluster_ctarank into its header, initialises its mbarriers, and after a cluster barrier reads
- * every peer's %smid through DSMEM, so that a record names both SMs of a transfer. Every word is compared bit for bit;
- * a wrong one is counted in the launch's gsb_cluster_log and nowhere else. Every mbarrier wait is a try_wait loop with a
- * %globaltimer deadline (GSB_CLUSTER_WAIT_NS); one that runs out is counted and the region checked anyway. Every CTA
- * ends with a cluster barrier, so none exits while a peer may still touch its shared memory.
+ * The kernel body and its device helpers are in gsb_cluster_body.inc, which the test-only twins
+ * (cluster_script_sm90a.cu) share.
  */
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -19,295 +15,11 @@
 
 namespace {
 
-constexpr uint32_t kThreads = 256;
-constexpr uint32_t kBulkChunk = 16384;  // bytes per cp.async.bulk instruction
-
-// The first GSB_CLUSTER_HEADER_BYTES of every CTA's dynamic shared memory.
-struct Header {
-  uint32_t smid, rank;
-  unsigned long long deadline[2];              // %globaltimer bounds: ST_ASYNC's free wait, the receive waits
-  uint32_t peer_smid[GSB_CLUSTER_MAX_N];       // %smid of every rank of the cluster, read through DSMEM
-  unsigned long long full[GSB_CLUSTER_MAX_N];  // per slot: the region's bytes have landed
-  unsigned long long free_bar;                 // ST_ASYNC: every peer's region for this CTA is ready
-};
-static_assert(sizeof(Header) <= GSB_CLUSTER_HEADER_BYTES, "header");
-
-__device__ __forceinline__ uint32_t smid() {
-  uint32_t s;
-  asm volatile("mov.u32 %0, %%smid;" : "=r"(s));
-  return s;
-}
-__device__ __forceinline__ uint32_t cluster_rank() {
-  uint32_t r;
-  asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(r));
-  return r;
-}
-__device__ __forceinline__ uint32_t cluster_size() {
-  uint32_t r;
-  asm volatile("mov.u32 %0, %%cluster_nctarank;" : "=r"(r));
-  return r;
-}
-__device__ __forceinline__ unsigned long long globaltimer() {
-  unsigned long long t;
-  asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t));
-  return t;
-}
-__device__ __forceinline__ uint32_t smem_u32(const void *p) { return (uint32_t)__cvta_generic_to_shared(p); }
-
-__device__ __forceinline__ void cluster_sync() {
-  asm volatile("barrier.cluster.arrive.release.aligned;\n\tbarrier.cluster.wait.acquire.aligned;" ::: "memory");
-}
-// the shared::cluster address of `addr` (a shared::cta address of this CTA) in the CTA of rank `rank`
-__device__ __forceinline__ uint32_t mapa(uint32_t addr, uint32_t rank) {
-  uint32_t r;
-  asm volatile("mapa.shared::cluster.u32 %0, %1, %2;" : "=r"(r) : "r"(addr), "r"(rank));
-  return r;
-}
-__device__ __forceinline__ uint4 lds(uint32_t addr) {
-  uint4 v;
-  asm volatile("ld.shared.v4.u32 {%0, %1, %2, %3}, [%4];" : "=r"(v.x), "=r"(v.y), "=r"(v.z), "=r"(v.w) : "r"(addr) : "memory");
-  return v;
-}
-__device__ __forceinline__ void sts(uint32_t addr, uint4 v) {
-  asm volatile("st.shared.v4.u32 [%0], {%1, %2, %3, %4};" ::"r"(addr), "r"(v.x), "r"(v.y), "r"(v.z), "r"(v.w) : "memory");
-}
-__device__ __forceinline__ uint4 ld_cluster(uint32_t addr) {
-  uint4 v;
-  asm volatile("ld.shared::cluster.v4.u32 {%0, %1, %2, %3}, [%4];" : "=r"(v.x), "=r"(v.y), "=r"(v.z), "=r"(v.w) : "r"(addr) : "memory");
-  return v;
-}
-__device__ __forceinline__ uint32_t ld_cluster_u32(uint32_t addr) {
-  uint32_t v;
-  asm volatile("ld.shared::cluster.u32 %0, [%1];" : "=r"(v) : "r"(addr) : "memory");
-  return v;
-}
-__device__ __forceinline__ void st_cluster(uint32_t addr, uint4 v) {
-  asm volatile("st.shared::cluster.v4.u32 [%0], {%1, %2, %3, %4};" ::"r"(addr), "r"(v.x), "r"(v.y), "r"(v.z), "r"(v.w) : "memory");
-}
-__device__ __forceinline__ void st_async(uint32_t addr, uint4 v, uint32_t mbar) {
-  asm volatile("st.async.shared::cluster.mbarrier::complete_tx::bytes.v4.b32 [%0], {%1, %2, %3, %4}, [%5];"
-               ::"r"(addr), "r"(v.x), "r"(v.y), "r"(v.z), "r"(v.w), "r"(mbar) : "memory");
-}
-__device__ __forceinline__ void mbar_init(uint32_t bar, uint32_t count) {
-  asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(bar), "r"(count) : "memory");
-}
-__device__ __forceinline__ void mbar_expect_tx(uint32_t bar, uint32_t bytes) {
-  asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(bar), "r"(bytes) : "memory");
-}
-// arrive on the mbarrier of a peer (`bar` a shared::cluster address), releasing this thread's prior writes
-__device__ __forceinline__ void mbar_arrive_remote(uint32_t bar) {
-  asm volatile("mbarrier.arrive.release.cluster.shared::cluster.b64 _, [%0];" ::"r"(bar) : "memory");
-}
-// phase 0 of `bar` complete by `deadline`? At least one try_wait before the deadline is looked at.
-__device__ __forceinline__ bool mbar_wait(uint32_t bar, unsigned long long deadline) {
-  for (;;) {
-    uint32_t ok;
-    asm volatile(
-        "{\n\t.reg .pred p;\n\t"
-        "mbarrier.try_wait.parity.acquire.cluster.shared::cta.b64 p, [%1], 0;\n\t"
-        "selp.u32 %0, 1, 0, p;\n\t}"
-        : "=r"(ok)
-        : "r"(bar)
-        : "memory");
-    if (ok) return true;
-    if (globaltimer() > deadline) return false;
-  }
-}
-__device__ __forceinline__ void bulk_s2s(uint32_t dst, uint32_t src, uint32_t bytes, uint32_t mbar) {
-  asm volatile("cp.async.bulk.shared::cluster.shared::cta.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];"
-               ::"r"(dst), "r"(src), "r"(bytes), "r"(mbar) : "memory");
-}
-__device__ __forceinline__ void bulk_multicast(uint32_t dst, const void *src, uint32_t bytes, uint32_t mbar,
-                                               uint16_t mask) {
-  asm volatile(
-      "cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes.multicast::cluster [%0], [%1], %2, [%3], %4;"
-      ::"r"(dst), "l"(src), "r"(bytes), "r"(mbar), "h"(mask) : "memory");
-}
-
-__device__ __forceinline__ uint4 word(uint64_t addr, uint32_t key) {
-  uint32_t l[4];
-  gsb_pattern_word(addr, key, l);
-  return make_uint4(l[0], l[1], l[2], l[3]);
-}
-
-__device__ __forceinline__ void set_bit(unsigned int *bitmap, uint32_t sm) {
-  if (sm < GSB_CLUSTER_SM_MAX) atomicOr(&bitmap[sm >> 5], 1u << (sm & 31u));
-}
-
-__device__ __noinline__ void mismatch(const gsb_cluster_args &a, const Header *h, uint32_t p, uint32_t n, uint32_t s,
-                                      uint32_t d, uint32_t i, uint4 e, uint4 o) {
-  gsb_cluster_log *log = a.log;
-  const uint32_t bits = __popc(e.x ^ o.x) + __popc(e.y ^ o.y) + __popc(e.z ^ o.z) + __popc(e.w ^ o.w);
-  atomicAdd(&log->mismatch_words, 1ull);
-  atomicAdd(&log->mismatch_bits, (unsigned long long)bits);
-  const uint32_t ss = h->peer_smid[s], ds = h->peer_smid[d];
-  set_bit(log->faulty, ss);
-  set_bit(log->faulty, ds);
-  const unsigned slot = atomicAdd(&log->count, 1u);
-  if (slot < GSB_CLUSTER_RECORDS) {
-    gsb_cluster_record &r = log->rec[slot];
-    r.path = p;
-    r.n = n;
-    r.src_rank = s;
-    r.dst_rank = d;
-    r.src_smid = ss;
-    r.dst_smid = ds;
-    r.index = i;
-    r.reserved0 = 0;
-    r.expected[0] = e.x, r.expected[1] = e.y, r.expected[2] = e.z, r.expected[3] = e.w;
-    r.observed[0] = o.x, r.observed[1] = o.y, r.observed[2] = o.z, r.observed[3] = o.w;
-  }
-}
-
-// words compared by the calling warp's threads (every thread of the warp calls it)
-__device__ __forceinline__ void add_words(gsb_cluster_log *log, uint32_t n) {
-  n = __reduce_add_sync(0xFFFFFFFFu, n);
-  if ((threadIdx.x & 31u) == 0) atomicAdd(&log->words, (unsigned long long)n);
-}
+#include "gsb_cluster_body.inc"
 
 template <uint32_t P>
 __global__ void __launch_bounds__(kThreads, 1) cluster_check(const gsb_cluster_args a) {
-  extern __shared__ __align__(128) unsigned char smem_raw[];
-  Header *h = reinterpret_cast<Header *>(smem_raw);
-  const uint32_t tid = threadIdx.x;
-  const uint32_t n = cluster_size(), rank = cluster_rank(), sm = smid();
-  const uint32_t area = smem_u32(smem_raw) + GSB_CLUSTER_HEADER_BYTES;
-  const uint32_t rw = gsb_cluster_region_words(P, n, a.smem_bytes), slots = gsb_cluster_slots(P, n);
-  const uint32_t send = area + 16u * slots * rw;  // BULK_S2S: the send tiles, by the receiver's slot in this area
-  const uint32_t key = gsb_seed_key(a.seed), key_expect = gsb_seed_key(a.seed_expect);
-  const uint32_t bg_key = gsb_cluster_bg_key(a.seed);
-  const bool skip = sm == a.skip_smid;
-  constexpr bool kMbar = P == GSB_CLUSTER_PATH_ST_ASYNC || P == GSB_CLUSTER_PATH_BULK_S2S ||
-                         P == GSB_CLUSTER_PATH_MULTICAST;
-  if (tid == 0) {
-    h->smid = sm;
-    h->rank = rank;
-    set_bit(a.log->covered, sm);
-    if constexpr (kMbar) {
-      for (uint32_t j = 0; j < slots; j++) mbar_init(smem_u32(&h->full[j]), 1u);
-      if constexpr (P == GSB_CLUSTER_PATH_ST_ASYNC) mbar_init(smem_u32(&h->free_bar), n - 1u);
-      asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-      // the bulk paths' senders start after the cluster barrier below, so every region is armed before a byte leaves
-      if constexpr (P != GSB_CLUSTER_PATH_ST_ASYNC)
-        for (uint32_t j = 0; j < slots; j++) mbar_expect_tx(smem_u32(&h->full[j]), 16u * rw);
-    }
-  }
-  // the area before anyone sends: its background (DSMEM_LD: the words the peers will read instead, unless skipped;
-  // BULK_S2S: the send tiles too). ST_ASYNC fills it after the barrier and then tells its peers with a remote arrive.
-  if constexpr (P != GSB_CLUSTER_PATH_ST_ASYNC) {
-    for (uint32_t j = 0; j < slots; j++) {
-      const uint32_t q = gsb_cluster_peer(P, n, rank, j);
-      for (uint32_t i = tid; i < rw; i += kThreads) {
-        const uint32_t w = j * rw + i;
-        const bool data = P == GSB_CLUSTER_PATH_DSMEM_LD && !skip;
-        sts(area + 16u * w, data ? word(gsb_cluster_word_addr(P, n, rank, q, i), key)
-                                 : word(gsb_cluster_bg_addr(P, n, rank, w), bg_key));
-        if (P == GSB_CLUSTER_PATH_BULK_S2S) sts(send + 16u * w, word(gsb_cluster_word_addr(P, n, rank, q, i), key));
-      }
-    }
-    // generic-proxy stores before the async proxy's reads (send tiles) and writes (regions)
-    if constexpr (P == GSB_CLUSTER_PATH_BULK_S2S || P == GSB_CLUSTER_PATH_MULTICAST)
-      asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
-  }
-  cluster_sync();
-  if (tid < n) h->peer_smid[tid] = ld_cluster_u32(mapa(smem_u32(&h->smid), tid));
-  __syncthreads();
-
-  uint32_t timeouts = 0;  // counted by thread 0 only
-  if constexpr (P == GSB_CLUSTER_PATH_DSMEM_ST) {
-    if (!skip) {
-      for (uint32_t j = 0; j + 1 < n; j++) {
-        const uint32_t q = (rank + 1u + j) % n;
-        const uint32_t dst = mapa(area + 16u * gsb_cluster_slot(P, n, q, rank) * rw, q);
-        for (uint32_t i = tid; i < rw; i += kThreads) st_cluster(dst + 16u * i, word(gsb_cluster_word_addr(P, n, rank, q, i), key));
-      }
-    }
-    cluster_sync();  // every store released to the cluster before the receivers look
-  }
-  if constexpr (P == GSB_CLUSTER_PATH_ST_ASYNC) {
-    for (uint32_t w = tid; w < slots * rw; w += kThreads) sts(area + 16u * w, word(gsb_cluster_bg_addr(P, n, rank, w), bg_key));
-    __syncthreads();
-    if (tid == 0) {
-      for (uint32_t j = 0; j < slots; j++) mbar_expect_tx(smem_u32(&h->full[j]), 16u * rw);
-      for (uint32_t j = 0; j < slots; j++) mbar_arrive_remote(mapa(smem_u32(&h->free_bar), gsb_cluster_peer(P, n, rank, j)));
-      h->deadline[0] = globaltimer() + GSB_CLUSTER_WAIT_NS;
-    }
-    __syncthreads();
-    const bool ready = mbar_wait(smem_u32(&h->free_bar), h->deadline[0]);  // every receiver's background is down
-    if (tid == 0 && !ready) timeouts++;
-    if (!skip) {
-      for (uint32_t j = 0; j + 1 < n; j++) {
-        const uint32_t q = (rank + 1u + j) % n, slot = gsb_cluster_slot(P, n, q, rank);
-        const uint32_t dst = mapa(area + 16u * slot * rw, q), bar = mapa(smem_u32(&h->full[slot]), q);
-        for (uint32_t i = tid; i < rw; i += kThreads) st_async(dst + 16u * i, word(gsb_cluster_word_addr(P, n, rank, q, i), key), bar);
-      }
-    }
-  }
-  if constexpr (P == GSB_CLUSTER_PATH_BULK_S2S) {
-    if (tid == 0 && !skip) {
-      for (uint32_t j = 0; j + 1 < n; j++) {
-        const uint32_t q = (rank + 1u + j) % n, slot = gsb_cluster_slot(P, n, q, rank);
-        const uint32_t dst = mapa(area + 16u * slot * rw, q), bar = mapa(smem_u32(&h->full[slot]), q);
-        const uint32_t src = send + 16u * gsb_cluster_slot(P, n, rank, q) * rw;
-        for (uint32_t b = 0; b < 16u * rw; b += kBulkChunk)
-          bulk_s2s(dst + b, src + b, min(kBulkChunk, 16u * rw - b), bar);
-      }
-    }
-  }
-  if constexpr (P == GSB_CLUSTER_PATH_MULTICAST) {
-    if (tid == 0 && !skip) {
-      const uint32_t dst = area + 16u * rank * rw, bar = smem_u32(&h->full[rank]);
-      const unsigned char *src = static_cast<const unsigned char *>(a.mc_src) + 16ull * rank * rw;
-      const uint16_t mask = (uint16_t)((1u << n) - 1u);
-      for (uint32_t b = 0; b < 16u * rw; b += kBulkChunk) bulk_multicast(dst + b, src + b, min(kBulkChunk, 16u * rw - b), bar, mask);
-    }
-  }
-  if constexpr (kMbar) {
-    if (tid == 0) h->deadline[1] = globaltimer() + GSB_CLUSTER_WAIT_NS;
-    __syncthreads();
-    for (uint32_t j = 0; j < slots; j++) {
-      const bool ok = mbar_wait(smem_u32(&h->full[j]), h->deadline[1]);
-      if (tid == 0 && !ok) timeouts++;
-    }
-  }
-
-  // the check: slot j of the receiver's view holds what peer q = gsb_cluster_peer(j) sent it
-  uint32_t checked = 0;
-  for (uint32_t j = 0; j < slots; j++) {
-    const uint32_t q = gsb_cluster_peer(P, n, rank, j);
-    const uint32_t d_addr = P == GSB_CLUSTER_PATH_MULTICAST ? GSB_CLUSTER_EVERY_RANK : rank;
-    uint32_t src = area + 16u * j * rw;
-    if constexpr (P == GSB_CLUSTER_PATH_DSMEM_LD) src = mapa(area + 16u * gsb_cluster_slot(P, n, q, rank) * rw, q);
-    for (uint32_t i = tid; i < rw; i += kThreads) {
-      uint4 o = P == GSB_CLUSTER_PATH_DSMEM_LD ? ld_cluster(src + 16u * i) : lds(src + 16u * i);
-      if (sm == a.hook_smid && j * rw + i == a.hook_index) {  // test hook
-        o.x ^= (uint32_t)a.hook_xr;
-        o.y ^= (uint32_t)(a.hook_xr >> 32);
-      }
-      const uint4 e = word(gsb_cluster_word_addr(P, n, q, d_addr, i), key_expect);
-      if (o.x != e.x || o.y != e.y || o.z != e.z || o.w != e.w) mismatch(a, h, P, n, q, rank, i, e, o);
-      checked++;
-    }
-  }
-  add_words(a.log, checked);
-  if (tid == 0 && timeouts) atomicAdd(&a.log->timeouts, timeouts);
-  cluster_sync();  // no CTA leaves while a peer may still read or write its shared memory
-}
-
-template <uint32_t P>
-cudaLaunchConfig_t config(uint32_t n, uint32_t clusters, uint32_t smem, cudaStream_t stream, cudaLaunchAttribute *attr) {
-  cudaLaunchConfig_t c = {};
-  c.gridDim = dim3(clusters * n, 1, 1);
-  c.blockDim = dim3(kThreads, 1, 1);
-  c.dynamicSmemBytes = smem;
-  c.stream = stream;
-  attr->id = cudaLaunchAttributeClusterDimension;
-  attr->val.clusterDim.x = n;
-  attr->val.clusterDim.y = 1;
-  attr->val.clusterDim.z = 1;
-  c.attrs = attr;
-  c.numAttrs = 1;
-  return c;
+  cluster_body<P, false>(a, nullptr);
 }
 
 template <uint32_t P>

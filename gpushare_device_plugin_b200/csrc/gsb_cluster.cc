@@ -35,6 +35,29 @@ bool same(const uint32_t a[4], const uint32_t b[4]) { return !memcmp(a, b, 16); 
 
 }  // namespace
 
+// Every mbarrier a script arms is owed exactly one sender's region: each slot of each area is filled at most once.
+bool gsb_cluster_script_valid(uint32_t p, uint32_t n, uint32_t region_words, const uint8_t *route) {
+  if (p >= GSB_CLUSTER_PATHS || n < 2 || n > GSB_CLUSTER_MAX_N || (n & (n - 1))) return false;
+  if (!route) return true;
+  if (!region_words || region_words > gsb_cluster_region_words(p, n, GSB_CLUSTER_SCRIPT_SMEM)) return false;
+  const uint32_t slots = gsb_cluster_slots(p, n);
+  uint32_t taken[GSB_CLUSTER_MAX_N] = {0};  // per area owner: the slots some pair lands in
+  for (uint32_t s = 0; s < n; s++) {
+    uint32_t row = GSB_CLUSTER_UNROUTED;
+    for (uint32_t d = 0; d < n; d++) {
+      const uint32_t t = route[s * n + d];
+      if (t == GSB_CLUSTER_UNROUTED) continue;
+      if (t >= slots || (s == d && p != GSB_CLUSTER_PATH_MULTICAST)) return false;
+      if (p == GSB_CLUSTER_PATH_MULTICAST && row != GSB_CLUSTER_UNROUTED && row != t) return false;
+      row = t;
+      const uint32_t owner = p == GSB_CLUSTER_PATH_DSMEM_LD ? s : d;
+      if (taken[owner] >> t & 1u) return false;
+      taken[owner] |= 1u << t;
+    }
+  }
+  return true;
+}
+
 extern "C" {
 
 // Only runs that launched count. A probe that launched nothing (its buffer could not be taken, the device was not

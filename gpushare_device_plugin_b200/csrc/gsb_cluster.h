@@ -58,4 +58,19 @@ GSB_HD uint64_t gsb_cluster_bg_addr(uint32_t p, uint32_t n, uint32_t o, uint32_t
 
 GSB_HD uint32_t gsb_cluster_bg_key(uint32_t seed) { return gsb_seed_key(seed ^ GSB_CLUSTER_BG_SALT); }
 
+/* the dynamic shared memory the hook's region sizes are bounded at: the H100's 227 KiB opt-in maximum */
+#define GSB_CLUSTER_SCRIPT_SMEM (GSB_CLUSTER_HEADER_BYTES + 16u * GSB_CLUSTER_HOOK_INDEX_MAX)
+
+/* gsb_test_cluster_script's script, as the twin kernels (cluster_script_sm90a.cu) read it from device memory: route is
+ * indexed s * n + d with the launch's n */
+typedef struct gsb_cluster_script {
+  uint32_t region_words;
+  uint8_t route[GSB_CLUSTER_MAX_N * GSB_CLUSTER_MAX_N];
+} gsb_cluster_script;
+
+#ifdef __cplusplus
+/* gsb_test_cluster_script's refusals (gsb_cluster.cc); route NULL checks the path and n only */
+bool gsb_cluster_script_valid(uint32_t p, uint32_t n, uint32_t region_words, const uint8_t *route);
+#endif
+
 #endif /* GSB_CLUSTER_H_ */

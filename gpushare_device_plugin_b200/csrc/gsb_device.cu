@@ -288,6 +288,12 @@ struct Device {
     uint64_t xr = 0;
   };
   CheckState<gsb_cluster_stats, std::array<ClusterHook, GSB_CLUSTER_PATHS>> cluster;  // hooks: gsb_test_cluster_*
+  // gsb_test_cluster_script, by path and size index (guarded by smu): taken by the next probe that runs the pair
+  struct ClusterScript {
+    bool armed = false;
+    gsb_cluster_script script = {};
+  };
+  std::array<std::array<ClusterScript, GSB_CLUSTER_SIZES>, GSB_CLUSTER_PATHS> cluster_scripts;
   // L2 atomic health
   struct AtomicHook {
     bool corrupt = false, skip = false;
@@ -561,6 +567,7 @@ int ensure_ready(Device *d) {
   if (pe == cudaSuccess) pe = (cudaError_t)gsb_sm_operands_preload(smem_optin);
   if (pe == cudaSuccess) pe = (cudaError_t)gsb_stress_kernel_preload(smem_optin);
   if (pe == cudaSuccess) pe = (cudaError_t)gsb_cluster_kernel_preload(smem_optin);
+  if (pe == cudaSuccess) pe = (cudaError_t)gsb_cluster_script_preload(smem_optin);
   if (pe == cudaSuccess) pe = (cudaError_t)gsb_atomic_kernel_preload(smem_optin);
   if (pe == cudaSuccess) pe = (cudaError_t)gsb_atomic_values_preload(smem_optin);
   if (pe == cudaSuccess) pe = (cudaError_t)gsb_tensor_kernel_preload(smem_optin);
@@ -2503,12 +2510,16 @@ constexpr uint32_t kClusterAllSizes = (1u << GSB_CLUSTER_SIZES) - 1;
 // a launch whose waits all run out takes two of them (ST_ASYNC: the free wait, then the receive waits)
 constexpr uint64_t kClusterWaitsMs = 2ull * GSB_CLUSTER_WAIT_NS / 1000000ull;
 
-// One SM-to-SM launch of `path`: `clusters` clusters of n CTAs.
+// One SM-to-SM launch of `path`: `clusters` clusters of n CTAs; with `script` (device memory), the path's test-only twin.
 int cluster_launch_locked(Device *d, uint32_t path, uint32_t n, uint32_t clusters, const gsb_cluster_args &args,
-                          gsb_cluster_log *log, uint64_t *kernel_ns) {
+                          const gsb_cluster_script *script, gsb_cluster_log *log, uint64_t *kernel_ns) {
   return sm_launch_locked(
-      d, "SM-to-SM check", [&] { return gsb_cluster_kernel_launch(path, n, clusters, &args, d->stream); }, args.log,
-      log, sizeof *log, kClusterWaitsMs, nullptr, kernel_ns);
+      d, "SM-to-SM check",
+      [&] {
+        return script ? gsb_cluster_script_launch(path, n, clusters, &args, script, d->stream)
+                      : gsb_cluster_kernel_launch(path, n, clusters, &args, d->stream);
+      },
+      args.log, log, sizeof *log, kClusterWaitsMs, nullptr, kernel_ns);
 }
 
 int cluster_probe_locked(Device *d, const gsb_cluster_cfg *cfg, gsb_cluster_result *out) {
@@ -2541,11 +2552,27 @@ int cluster_probe_locked(Device *d, const gsb_cluster_cfg *cfg, gsb_cluster_resu
   out->seed = seed_or_fresh(cfg->seed, 0x434C0000u, &d->cluster.seed);
   out->seed_expect = cfg->seed_expect ? cfg->seed_expect : out->seed;
   auto hooks = take_hooks(d, &d->cluster.hooks);
-  // one transient buffer: the launch log, then the multicast source (n segments; at most the area of one CTA)
+  // gsb_test_cluster_script: taken by the first probe that runs its (path, size)
+  std::array<std::array<Device::ClusterScript, GSB_CLUSTER_SIZES>, GSB_CLUSTER_PATHS> scripts;
+  bool any_script = false;
+  {
+    std::lock_guard<std::mutex> lk(d->smu);
+    for (uint32_t p = 0; p < GSB_CLUSTER_PATHS; p++)
+      for (uint32_t k = 0; k < GSB_CLUSTER_SIZES; k++)
+        if (out->paths >> p & 1u && out->sizes >> k & 1u && d->cluster_scripts[p][k].armed) {
+          scripts[p][k] = std::exchange(d->cluster_scripts[p][k], Device::ClusterScript{});
+          any_script = true;
+        }
+  }
+  // one transient buffer: the launch log, then the multicast source (n segments; at most the area of one CTA), then
+  // with a script, the script and its own multicast source
   const size_t log_bytes = (sizeof(gsb_cluster_log) + 255) / 256 * 256;
   const size_t src_bytes = 16ull * gsb_cluster_area_words((uint32_t)smem);
+  const size_t script_bytes = (sizeof(gsb_cluster_script) + 255) / 256 * 256;
   SmBuffer buf(d, rc);
-  rc = buf.alloc("SM-to-SM probe", log_bytes + src_bytes);
+  rc = buf.alloc("SM-to-SM probe", log_bytes + src_bytes + (any_script ? script_bytes + src_bytes : 0));
+  gsb_cluster_script *script_dev = reinterpret_cast<gsb_cluster_script *>(static_cast<char *>(buf.p) + log_bytes + src_bytes);
+  const void *script_src = static_cast<char *>(buf.p) + log_bytes + src_bytes + script_bytes;
   std::vector<uint32_t> src_words;
   for (uint32_t k = 0; k < GSB_CLUSTER_SIZES && rc == GSB_OK; k++) {
     if (!(out->sizes >> k & 1u)) continue;
@@ -2565,20 +2592,34 @@ int cluster_probe_locked(Device *d, const gsb_cluster_cfg *cfg, gsb_cluster_resu
       a.seed = out->seed;
       a.seed_expect = out->seed_expect;
       a.smem_bytes = (uint32_t)smem;
-      if (p == GSB_CLUSTER_PATH_MULTICAST) {  // segment s: what rank s multicasts to every rank
-        const uint32_t rw = gsb_cluster_region_words(p, n, (uint32_t)smem), key = gsb_seed_key(out->seed);
+      const Device::ClusterScript &sc = scripts[p][k];
+      if (sc.armed && sc.script.region_words > gsb_cluster_region_words(p, n, (uint32_t)smem)) {
+        set_error("an SM-to-SM script of %u words per region does not fit %d bytes of shared memory on %s",
+                  sc.script.region_words, smem, d->uuid);
+        run.status = rc = GSB_ERR_INVALID_ARGUMENT;
+        break;
+      }
+      // segment s: what rank s multicasts to every rank, at the probe's region size and at the script's
+      const auto upload = [&](const void *dst, uint32_t rw) {
+        const uint32_t key = gsb_seed_key(out->seed);
         src_words.resize(4ull * n * rw);
         for (uint32_t s = 0; s < n; s++)
           for (uint32_t i = 0; i < rw; i++)
             gsb_pattern_word(gsb_cluster_word_addr(p, n, s, GSB_CLUSTER_EVERY_RANK, i), key,
                              &src_words[4ull * (s * rw + i)]);
-        const cudaError_t e = cudaMemcpyAsync(const_cast<void *>(a.mc_src), src_words.data(), 4 * src_words.size(),
-                                              cudaMemcpyHostToDevice, d->stream);
-        if (e != cudaSuccess || cudaStreamSynchronize(d->stream) != cudaSuccess) {
-          set_error("uploading the SM-to-SM probe's multicast source to %s: %s", d->uuid, cudaGetErrorString(e));
-          run.status = rc = GSB_ERR_DRIVER;
-          break;
-        }
+        return cudaMemcpyAsync(const_cast<void *>(dst), src_words.data(), 4 * src_words.size(), cudaMemcpyHostToDevice,
+                               d->stream);
+      };
+      cudaError_t e = cudaSuccess;
+      if (p == GSB_CLUSTER_PATH_MULTICAST) e = upload(a.mc_src, gsb_cluster_region_words(p, n, (uint32_t)smem));
+      if (e == cudaSuccess && sc.armed && p == GSB_CLUSTER_PATH_MULTICAST) e = upload(script_src, sc.script.region_words);
+      if (e == cudaSuccess && sc.armed)
+        e = cudaMemcpyAsync(script_dev, &sc.script, sizeof sc.script, cudaMemcpyHostToDevice, d->stream);
+      if (e != cudaSuccess || (e = cudaStreamSynchronize(d->stream)) != cudaSuccess) {
+        set_error("uploading the SM-to-SM probe's multicast source or script to %s: %s", d->uuid,
+                  cudaGetErrorString(e));
+        run.status = rc = GSB_ERR_DRIVER;
+        break;
       }
       uint32_t covered[GSB_CLUSTER_SM_MAX / 32] = {0};
       // a launch that left an SM it could reach uncovered (another context held it) is repeated
@@ -2591,9 +2632,14 @@ int cluster_probe_locked(Device *d, const gsb_cluster_cfg *cfg, gsb_cluster_resu
         }
         if (hooks[p].skip) a.skip_smid = hooks[p].skip_smid;
         hooks[p] = Device::ClusterHook{};
+        // a script runs in the pair's first launch only; a relaunch for coverage is the probe's own
+        const bool scripted = sc.armed && run.launches == 0;
+        gsb_cluster_args la = a;
+        if (scripted && p == GSB_CLUSTER_PATH_MULTICAST) la.mc_src = script_src;
         run.launches++;
         gsb_cluster_log log;
-        const int lrc = cluster_launch_locked(d, p, n, out->max_clusters[k], a, &log, &run.kernel_ns);
+        const int lrc = cluster_launch_locked(d, p, n, out->max_clusters[k], la, scripted ? script_dev : nullptr, &log,
+                                              &run.kernel_ns);
         if (lrc != GSB_OK) {
           run.status = rc = lrc;
           break;
@@ -4264,6 +4310,23 @@ int gsb_test_cluster_skip(uint32_t idx, uint32_t smid, uint32_t path) {
   Device::ClusterHook &h = d->cluster.hooks[path];
   h.skip = true;
   h.skip_smid = smid;
+  return GSB_OK;
+}
+
+int gsb_test_cluster_script(uint32_t idx, uint32_t path, uint32_t n, uint32_t region_words, const uint8_t *route) {
+  std::shared_lock<std::shared_mutex> api_lk(G.api_mu);
+  if (!gsb_cluster_script_valid(path, n, region_words, route)) return GSB_ERR_INVALID_ARGUMENT;  // before any device
+  Device *d = device_at(idx);
+  if (!d) return G.inited ? GSB_ERR_NO_DEVICE : GSB_ERR_NOT_INITIALIZED;
+  Device::ClusterScript sc;
+  if (route) {
+    sc.armed = true;
+    sc.script.region_words = region_words;
+    memset(sc.script.route, GSB_CLUSTER_UNROUTED, sizeof sc.script.route);
+    memcpy(sc.script.route, route, (size_t)n * n);
+  }
+  std::lock_guard<std::mutex> lk(d->smu);
+  d->cluster_scripts[path][__builtin_ctz(n) - 1] = sc;
   return GSB_OK;
 }
 

@@ -362,6 +362,12 @@ int gsb_cluster_max_active(uint32_t n, int smem_bytes, int *clusters);
 /* Load the SM-to-SM kernels into the CURRENT context, let each take `smem_bytes` of dynamic shared memory and allow
  * clusters of 16. */
 int gsb_cluster_kernel_preload(int smem_bytes);
+/* gsb_test_cluster_script: enqueue the test-only twin of `path`'s launch (cluster_script_sm90a.cu, in
+ * libgpushare_b200_cluster_script.so), its region size and
+ * routes read from `s` in device memory. Returns cudaError_t as int. */
+int gsb_cluster_script_launch(uint32_t path, uint32_t n, uint32_t clusters, const gsb_cluster_args *a,
+                              const struct gsb_cluster_script *s, cudaStream_t stream);
+int gsb_cluster_script_preload(int smem_bytes);
 
 /* What one L2 atomic launch (atomic_check_sm90a.cu) leaves in device memory; the host zeroes it before every launch.
  * A run launch fills the first part, a check launch the counts and records. */

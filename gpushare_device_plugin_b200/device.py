@@ -631,8 +631,24 @@ def test_cluster_skip(idx: int, smid: int, path: int) -> None:
     check(lib.gsb_test_cluster_skip(idx, smid, path), f"gsb_test_cluster_skip({idx})")
 
 
+def test_cluster_script(idx: int, path: int, n: int, region_words: int, route) -> None:
+    """Test hook: the first launch of (`path`, clusters of `n`) in the next SM-to-SM probe of `idx` that runs that pair
+    is the path's twin on a script: regions of `region_words` words, and the words of rank s for rank d in slot
+    route[s][d] of their area (n x n, or n * n flat; GSB_CLUSTER_UNROUTED: nowhere); once. route=None disarms it."""
+    import numpy as np
+    if route is None:
+        check(lib.gsb_test_cluster_script(idx, path, n, region_words, None), f"gsb_test_cluster_script({idx})")
+        return
+    r = np.ascontiguousarray(route, dtype=np.uint8).reshape(-1)
+    if r.size != n * n:
+        raise ValueError(f"test_cluster_script: route has {r.size} entries, not {n} x {n}")
+    check(lib.gsb_test_cluster_script(idx, path, n, region_words, r.ctypes.data_as(C.POINTER(C.c_uint8))),
+          f"gsb_test_cluster_script({idx})")
+
+
 test_cluster_corrupt.__test__ = False
 test_cluster_skip.__test__ = False
+test_cluster_script.__test__ = False
 
 
 def atomic_probe(idx: int, *, ops: int = 0, seed: int = 0, seed_expect: int = 0,

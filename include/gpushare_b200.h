@@ -1193,6 +1193,17 @@ int gsb_test_cluster_corrupt(uint32_t idx, uint32_t smid, uint32_t path, uint32_
  * nothing (DSMEM_LD: leaves its area's background for its readers); its receivers find STALE words and, on the mbarrier
  * paths, a wait that runs out; once */
 int gsb_test_cluster_skip(uint32_t idx, uint32_t smid, uint32_t path);
+#define GSB_CLUSTER_UNROUTED 0xFFu /* gsb_test_cluster_script: rank s sends rank d nothing */
+/* test hook: the first launch of (path, n) in the next gsb_cluster_probe of device idx that runs that pair is the
+ * path's test-only twin, run on a script; once. Every region is region_words words (1 up to the path's region words at
+ * n with the 227 KiB opt-in maximum) and route[s * n + d] (n x n bytes) is the slot, in the area the words of rank s for
+ * rank d land in (d's; DSMEM_LD: s's own), where they go, or GSB_CLUSTER_UNROUTED. A receiver arms and waits on the
+ * mbarriers of routed slots only; the compare is the probe's own, so a word routed elsewhere is MISROUTED and a slot
+ * nobody fills is STALE. MULTICAST: row s is one slot or GSB_CLUSTER_UNROUTED throughout, and the ranks it names are
+ * the multicast mask. Refused before any device is touched: an unknown path, n not 2, 4, 8 or 16, region_words out of
+ * range, a slot past the path's slots, s routed to itself (but on MULTICAST), two senders in one slot of one area, a
+ * MULTICAST row with two slots. route NULL disarms it. Later launches of the pair (coverage) are the probe's own. */
+int gsb_test_cluster_script(uint32_t idx, uint32_t path, uint32_t n, uint32_t region_words, const uint8_t *route);
 
 /* ---- L2 atomic health (not in the reference; opt-in: GSB_OPT_ATOMIC_PROBE_EVERY_CYCLES) ---------------------------- */
 

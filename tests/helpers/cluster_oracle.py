@@ -28,7 +28,10 @@ def slots(p: int, n: int) -> int:
     return n if p == MULTICAST else n - 1
 
 
-def region_words(p: int, n: int, smem_bytes: int) -> int:
+def region_words(p: int, n: int, smem_bytes: int, rw: int | None = None) -> int:
+    """Words of every region; `rw` overrides the probe's geometry (a script's region size)."""
+    if rw is not None:
+        return rw
     aw = area_words(smem_bytes) // (2 if p == BULK_S2S else 1)
     return aw // slots(p, n) // 8 * 8
 
@@ -80,23 +83,25 @@ def background(seed: int, p: int, n: int, owner: int, j) -> np.ndarray:
     return words(bg_addr(p, n, owner, j), bg_key(seed))
 
 
-def stale(seed: int, p: int, n: int, s: int, d: int, i, smem_bytes: int) -> np.ndarray:
+def stale(seed: int, p: int, n: int, s: int, d: int, i, smem_bytes: int, rw: int | None = None) -> np.ndarray:
     """What receiver d reads at word i of sender s's region when s sent nothing: the background of the area read."""
-    rw = region_words(p, n, smem_bytes)
+    rw = region_words(p, n, smem_bytes, rw)
     owner, other = (s, d) if p == DSMEM_LD else (d, s)
     return background(seed, p, n, owner, slot(p, n, owner, other) * rw + np.asarray(i))
 
 
-def classify(seed: int, smem_bytes: int, p: int, n: int, s: int, d: int, i: int, expected, observed) -> dict:
-    """What the wrong word at (p, n, s, d, i) holds: cls, and for MISROUTED the pair and index it belongs to."""
+def classify(seed: int, smem_bytes: int, p: int, n: int, s: int, d: int, i: int, expected, observed,
+             rw: int | None = None) -> dict:
+    """What the wrong word at (p, n, s, d, i) holds: cls, and for MISROUTED the pair and index it belongs to. `rw`:
+    the launch's region size, when it is not the probe's."""
     e, o = np.asarray(expected, dtype=np.uint32), np.asarray(observed, dtype=np.uint32)
     out = {"cls": BITS, "src_rank": 0, "dst_rank": 0, "index": 0,
            "flipped_bits": int(sum(bin(int(x)).count("1") for x in (e ^ o)))}
     if not o.any():
         return dict(out, cls=ZERO)
-    if (stale(seed, p, n, s, d, i, smem_bytes)[0] == o).all():
+    if (stale(seed, p, n, s, d, i, smem_bytes, rw)[0] == o).all():
         return dict(out, cls=STALE)
-    rw = region_words(p, n, smem_bytes)
+    rw = region_words(p, n, smem_bytes, rw)
     idx = np.arange(rw, dtype=np.uint64)
     pairs = [(a, EVERY) for a in range(n)] if p == MULTICAST else [(a, b) for a in range(n) for b in range(n) if a != b]
     for a, b in pairs:
