@@ -87,6 +87,13 @@ TENSOR_UNIT_NAMES = ["dmma", "tf32", "e5m2", "e4m3_e5m2", "e5m2_e4m3", "f16_acc"
 GSB_TENSOR_UNITS, GSB_TENSOR_RECORDS, GSB_TENSOR_MAX_LAUNCHES, GSB_TENSOR_WORDS = 8, 64, 3, 8192
 GSB_TENSOR_CORRUPT, GSB_TENSOR_FAILED = 1, 2
 TENSOR_CONDITION_NAMES = {1: "wrong tensor-core result", 2: "tensor probe failed"}
+GSB_SPARSE_UNIT_F16_SP, GSB_SPARSE_UNIT_BF16_SP, GSB_SPARSE_UNIT_TF32_SP, GSB_SPARSE_UNIT_E4M3_SP, \
+    GSB_SPARSE_UNIT_E5M2_SP, GSB_SPARSE_UNIT_S8_SP, GSB_SPARSE_UNIT_HMMA_SP = range(7)
+SPARSE_UNIT_NAMES = ["f16", "bf16", "tf32", "e4m3", "e5m2", "s8", "hmma"]
+SPARSE_UNIT_K = [512, 512, 256, 128, 128, 512, 512]  # logical K of each unit (= gsb_sparse_shape(unit).k)
+GSB_SPARSE_UNITS, GSB_SPARSE_RECORDS, GSB_SPARSE_MAX_LAUNCHES, GSB_SPARSE_WORDS = 7, 64, 3, 8192
+GSB_SPARSE_CORRUPT, GSB_SPARSE_FAILED = 1, 2
+SPARSE_CONDITION_NAMES = {1: "wrong sparse tensor-core result", 2: "sparse probe failed"}
 GSB_SFU_UNIT_CVT_HALF, GSB_SFU_UNIT_CVT_FP8, GSB_SFU_UNIT_CVT_INT, GSB_SFU_UNIT_DIVSQRT, GSB_SFU_UNIT_WARP, \
     GSB_SFU_UNIT_MUFU = range(6)
 SFU_UNIT_NAMES = ["cvt_half", "cvt_fp8", "cvt_int", "divsqrt", "warp", "mufu"]
@@ -138,8 +145,9 @@ GSB_VARIANT_AUTO, GSB_VARIANT_DIRECT, GSB_VARIANT_CPASYNC, GSB_VARIANT_BULK, GSB
 VARIANT_NAMES = {0: "auto", 1: "direct", 2: "cpasync", 3: "bulk", 4: "bulkw", 5: "bulkd"}
 GSB_PROBE_TIMED, GSB_PROBE_SEED_TABLE = 1, 2
 GSB_EVENT_XID, GSB_EVENT_PROBE, GSB_EVENT_INVENTORY, GSB_EVENT_ECC, GSB_EVENT_LINK, GSB_EVENT_COPY, GSB_EVENT_SM, \
-    GSB_EVENT_CLUSTER, GSB_EVENT_ATOMIC, GSB_EVENT_TENSOR, GSB_EVENT_SFU, GSB_EVENT_L1, GSB_EVENT_ORDER = 8, 0x100, 0x200, \
-    0x400, 0x800, 0x1000, 0x2000, 0x4000, 0x8000, 0x10000, 0x20000, 0x40000, 0x80000
+    GSB_EVENT_CLUSTER, GSB_EVENT_ATOMIC, GSB_EVENT_TENSOR, GSB_EVENT_SFU, GSB_EVENT_L1, GSB_EVENT_ORDER, \
+    GSB_EVENT_SPARSE = 8, 0x100, 0x200, 0x400, 0x800, 0x1000, 0x2000, 0x4000, 0x8000, 0x10000, 0x20000, 0x40000, \
+    0x80000, 0x100000
 GSB_PROBE_FAULT_MISMATCH, GSB_PROBE_FAULT_LAUNCH, GSB_PROBE_RECOVERED, GSB_PROBE_FAULT_WEDGED = 1, 2, 3, 4
 GSB_INVENTORY_IDENTITY_CHANGED, GSB_INVENTORY_TOTAL_CHANGED = 1, 2
 GSB_ECC_VALID_MODE, GSB_ECC_VALID_VOLATILE, GSB_ECC_VALID_AGGREGATE, GSB_ECC_VALID_DRAM, GSB_ECC_VALID_REMAP, \
@@ -158,7 +166,8 @@ GSB_OPT_INVENTORY_POLICY, GSB_OPT_WAIT_SPIN_US, GSB_OPT_WATCHDOG_MS, GSB_OPT_INV
     GSB_OPT_TRANSIENT_KEEP_FREE_BYTES, GSB_OPT_SWEEP_EVERY_CYCLES, GSB_OPT_ECC_HEALTH, GSB_OPT_LINK_PROBE_EVERY_CYCLES, \
     GSB_OPT_COPY_PROBE_EVERY_CYCLES, GSB_OPT_SM_PROBE_EVERY_CYCLES, GSB_OPT_CLUSTER_PROBE_EVERY_CYCLES, \
     GSB_OPT_ATOMIC_PROBE_EVERY_CYCLES, GSB_OPT_TENSOR_PROBE_EVERY_CYCLES, GSB_OPT_SFU_PROBE_EVERY_CYCLES, \
-    GSB_OPT_L1_PROBE_EVERY_CYCLES, GSB_OPT_ORDER_PROBE_EVERY_CYCLES = 1, 2, 3, 4, 5, 6, 7, 8, 9, 10, 11, 12, 13, 14, 15, 16
+    GSB_OPT_L1_PROBE_EVERY_CYCLES, GSB_OPT_ORDER_PROBE_EVERY_CYCLES, GSB_OPT_SPARSE_PROBE_EVERY_CYCLES = \
+    1, 2, 3, 4, 5, 6, 7, 8, 9, 10, 11, 12, 13, 14, 15, 16, 17
 GSB_INVENTORY_SNAPSHOT, GSB_INVENTORY_LIVE = 0, 1
 GSB_ALLOC_MATCHED, GSB_ALLOC_SINGLE_GPU, GSB_ALLOC_ERR_RESPONSE = 1, 2, 3
 UINT64_MAX = (1 << 64) - 1
@@ -194,6 +203,8 @@ SYMBOLS = [
     "gsb_test_l1_skip", "gsb_test_l1_table",
     "gsb_order_probe", "gsb_order_stats_get", "gsb_order_distance", "gsb_order_iriw_distance", "gsb_order_pairing",
     "gsb_order_classify", "gsb_order_conditions", "gsb_order_text", "gsb_test_order_inject", "gsb_test_order_skip",
+    "gsb_sparse_probe", "gsb_sparse_stats_get", "gsb_sparse_expected", "gsb_sparse_conditions", "gsb_sparse_text",
+    "gsb_test_sparse_corrupt", "gsb_test_sparse_operands",
     "gsb_allocate", "gsb_allocate_err_response", "gsb_patch_assigned_body",
 ]
 
@@ -851,6 +862,38 @@ class TensorStats(C.Structure):
     ]
 
 
+SparseCfg = TensorCfg  # the same four fields
+
+
+class SparseResult(C.Structure):
+    _fields_ = [
+        ("status", C.c_int32),
+        ("sm_count", C.c_uint32),
+        ("seed", C.c_uint32),
+        ("seed_expect", C.c_uint32),
+        ("units", C.c_uint32),
+        ("sms_covered", C.c_uint32),
+        ("covered", C.c_uint32 * (GSB_SM_MAX // 32)),
+        ("faulty", C.c_uint32 * (GSB_SM_MAX // 32)),
+        ("unit", TensorUnitResult * GSB_SPARSE_UNITS),
+        ("n_records", C.c_uint32),
+        ("reserved0", C.c_uint32),
+        ("records", SmRecord * GSB_SPARSE_RECORDS),  # unit: GSB_SPARSE_UNIT_*
+        ("expected_ns", C.c_uint64),
+        ("wall_ns", C.c_uint64),
+    ]
+
+
+class SparseStats(C.Structure):
+    _fields_ = [
+        ("probes", C.c_uint64),
+        ("faults", C.c_uint64),
+        ("skipped", C.c_uint64),
+        ("incomplete", C.c_uint64),
+        ("last", SparseResult),
+    ]
+
+
 class SfuCfg(C.Structure):
     _fields_ = [
         ("seed", C.c_uint32),
@@ -1205,6 +1248,13 @@ def _load() -> C.CDLL:
         "gsb_order_text": (C.c_int64, [C.POINTER(OrderResult), C.c_char_p, C.c_char_p, C.c_size_t]),
         "gsb_test_order_inject": (C.c_int, [C.c_uint32] * 4),
         "gsb_test_order_skip": (C.c_int, [C.c_uint32, C.c_uint32]),
+        "gsb_sparse_probe": (C.c_int, [C.c_uint32, C.POINTER(SparseCfg), C.POINTER(SparseResult)]),
+        "gsb_sparse_stats_get": (C.c_int, [C.c_uint32, C.POINTER(SparseStats)]),
+        "gsb_sparse_expected": (C.c_int64, [C.c_uint32, C.c_uint32, u32p, C.c_size_t]),
+        "gsb_sparse_conditions": (C.c_uint32, [C.POINTER(SparseResult)]),
+        "gsb_sparse_text": (C.c_int64, [C.POINTER(SparseResult), C.c_char_p, C.c_char_p, C.c_size_t]),
+        "gsb_test_sparse_corrupt": (C.c_int, [C.c_uint32, C.c_uint32, C.c_uint32, C.c_uint32, C.c_uint64]),
+        "gsb_test_sparse_operands": (C.c_int, [C.c_uint32, C.c_uint32, i32p, u8p, i32p, i32p, i32p, u64p]),
         "gsb_allocate": (C.c_int, [C.POINTER(AllocateCtx), C.POINTER(Pod), C.c_uint32, C.c_char_p, C.c_size_t, C.c_void_p, C.c_size_t, C.POINTER(C.c_size_t), C.POINTER(C.c_int32), u32p]),
         "gsb_allocate_err_response": (C.c_int, [C.POINTER(AllocateCtx), C.c_char_p, C.c_size_t, C.c_void_p, C.c_size_t, C.POINTER(C.c_size_t)]),
         "gsb_patch_assigned_body": (C.c_int, [C.c_uint64, C.c_char_p, C.c_size_t]),

@@ -174,6 +174,14 @@ const Check kChecks[] = {
       {GSB_ORDER_TIMEOUT, "grid barrier ran out"},
       {GSB_ORDER_FAILED, "memory-ordering probe failed"}},
      "memory-ordering condition ?"},
+    {&Flags::probe_sparse_every, GSB_OPT_SPARSE_PROBE_EVERY_CYCLES, GSB_EVENT_SPARSE, "sparse tensor-core health",
+     "sparse",
+     [](uint32_t i, const std::string &u) {
+       return probed<gsb_sparse_stats>(i, u, gsb_sparse_stats_get, gsb_sparse_text, nullptr,
+                                       &gsb_sparse_stats::incomplete);
+     },
+     {{GSB_SPARSE_CORRUPT, "wrong sparse tensor-core result"}, {GSB_SPARSE_FAILED, "sparse probe failed"}},
+     "sparse condition ?"},
 };
 constexpr size_t kNumChecks = sizeof kChecks / sizeof kChecks[0];
 

@@ -54,6 +54,7 @@
 #include "gsb_sfu_kat.h"
 #include "gsb_l1.h"
 #include "gsb_order.h"
+#include "gsb_sparse_kat.h"
 
 namespace {
 
@@ -343,6 +344,13 @@ struct Device {
     uint32_t skip_smid = 0;
   };
   CheckState<gsb_order_stats, OrderHooks> order;
+  // sparse tensor-core health: gsb_test_sparse_corrupt, and gsb_test_sparse_operands' expected words then its operand
+  // table (gsb_sparse_table_*), by GSB_SPARSE_UNIT_*; empty = not armed
+  struct SparseHooks {
+    std::array<SmCorrupt, GSB_SPARSE_UNITS> corrupt;
+    std::vector<uint32_t> operands[GSB_SPARSE_UNITS];
+  };
+  CheckState<gsb_sparse_stats, SparseHooks> sparse;
 
   // persistent worker (gsb_cycle_all / gsb_probe_all): one host thread per device
   std::thread worker;
@@ -372,7 +380,7 @@ struct Global {
   std::atomic<uint64_t> transient_keep_free{1ull << 30};
   std::atomic<uint64_t> sweep_every{0};
   std::atomic<uint64_t> ecc_health{0};
-  std::atomic<uint64_t> check_every[9] = {};  // GSB_OPT_*_PROBE_EVERY_CYCLES, by the check's place in Checks
+  std::atomic<uint64_t> check_every[10] = {};  // GSB_OPT_*_PROBE_EVERY_CYCLES, by the check's place in Checks
 
   // one link or copy probe's pinned buffers at a time in the whole process (the DaemonSet's memory limit covers 8 GPUs)
   std::mutex link_mu;
@@ -576,6 +584,8 @@ int ensure_ready(Device *d) {
   if (pe == cudaSuccess) pe = (cudaError_t)gsb_l1_kernel_preload();
   if (pe == cudaSuccess) pe = (cudaError_t)gsb_sfu_operands_preload(smem_optin);
   if (pe == cudaSuccess) pe = (cudaError_t)gsb_order_kernel_preload(smem_optin);
+  if (pe == cudaSuccess) pe = (cudaError_t)gsb_sparse_kernel_preload(smem_optin);
+  if (pe == cudaSuccess) pe = (cudaError_t)gsb_sparse_operands_preload(smem_optin);
   if (pe != cudaSuccess) {
     set_error("loading the probe kernels on %s: %s", d->uuid, cudaGetErrorString(pe));
     return (pe == cudaErrorInvalidDeviceFunction || pe == cudaErrorNoKernelImageForDevice) ? GSB_ERR_UNSUPPORTED_ARCH
@@ -3508,6 +3518,122 @@ int order_probe_locked(Device *d, const gsb_order_cfg *cfg, gsb_order_result *ou
   return rc;
 }
 
+// ------------------------------------------------------------------ sparse tensor-core health
+
+constexpr uint32_t kSparseAllUnits = (1u << GSB_SPARSE_UNITS) - 1;
+
+int sparse_probe_locked(Device *d, const gsb_sparse_cfg *cfg, gsb_sparse_result *out) {
+  const uint64_t t0 = now_ns();
+  if (cfg->units & ~kSparseAllUnits) {
+    set_error("invalid sparse unit mask 0x%x", cfg->units);
+    return out->status = GSB_ERR_INVALID_ARGUMENT;
+  }
+  out->units = cfg->units ? cfg->units : kSparseAllUnits;
+  out->sm_count = d->sm_count;
+  int rc = ensure_ready(d);
+  if (!rc) rc = sm_drain_kept_locked(d);
+  if (rc) return out->status = rc;
+  out->seed = seed_or_fresh(cfg->seed, 0x53500000u, &d->sparse.seed);
+  out->seed_expect = cfg->seed_expect ? cfg->seed_expect : out->seed;
+  const auto corrupt = take_hooks(d, &d->sparse.hooks.corrupt);
+  std::vector<uint32_t> chosen[GSB_SPARSE_UNITS];  // gsb_test_sparse_operands of the units this probe runs
+  {
+    std::lock_guard<std::mutex> lk(d->smu);
+    for (uint32_t u = 0; u < GSB_SPARSE_UNITS; u++)
+      if (out->units >> u & 1u) chosen[u].swap(d->sparse.hooks.operands[u]);
+  }
+  // the buffer: the launch log, then per unit its 8192 expected words or its chosen operands' block, 256-byte aligned
+  size_t offset[GSB_SPARSE_UNITS] = {}, bytes = (sizeof(gsb_sm_log) + 255) / 256 * 256;
+  for (uint32_t u = 0; u < GSB_SPARSE_UNITS; u++) {
+    if (!(out->units >> u & 1u)) continue;
+    offset[u] = bytes;
+    const size_t n = chosen[u].empty() ? (size_t)GSB_SPARSE_WORDS : chosen[u].size();
+    bytes += (n * sizeof(uint32_t) + 255) / 256 * 256;
+  }
+  // the exact answers, computed on the host; HMMA_SP's is F16_SP's
+  const uint64_t t_exp = now_ns();
+  std::string tables(bytes, '\0');
+  std::vector<uint32_t> f16;
+  for (uint32_t u = 0; u < GSB_SPARSE_UNITS; u++) {
+    if (!(out->units >> u & 1u)) continue;
+    uint32_t *p = reinterpret_cast<uint32_t *>(&tables[offset[u]]);
+    if (!chosen[u].empty()) {
+      memcpy(p, chosen[u].data(), chosen[u].size() * sizeof(uint32_t));
+      continue;
+    }
+    const bool f16_gemm = u == GSB_SPARSE_UNIT_F16_SP || u == GSB_SPARSE_UNIT_HMMA_SP;
+    if (f16_gemm && !f16.empty()) {
+      memcpy(p, f16.data(), GSB_SPARSE_WORDS * sizeof(uint32_t));
+    } else {
+      gsb_sparse_expected(u, out->seed_expect, p, GSB_SPARSE_WORDS);
+      if (f16_gemm) f16.assign(p, p + GSB_SPARSE_WORDS);
+    }
+  }
+  out->expected_ns = now_ns() - t_exp;
+  // one transient buffer: the launch log and the tables, under the keep-free margin of every transient probe
+  SmBuffer buf(d, rc);
+  rc = buf.alloc("sparse probe", bytes);
+  char *const base = static_cast<char *>(buf.p);
+  if (rc == GSB_OK) {
+    const size_t head = (sizeof(gsb_sm_log) + 255) / 256 * 256;
+    const cudaError_t e = cudaMemcpyAsync(base + head, &tables[head], bytes - head, cudaMemcpyHostToDevice, d->stream);
+    if (e != cudaSuccess || cudaStreamSynchronize(d->stream) != cudaSuccess) {
+      set_error("uploading the sparse probe's expected answers to %s: %s", d->uuid, cudaGetErrorString(e));
+      rc = GSB_ERR_DRIVER;
+    }
+  }
+  int smem = 0;
+  if (rc == GSB_OK) rc = smem_optin_locked(d, &smem);
+  bool first = true;
+  for (uint32_t u = 0; u < GSB_SPARSE_UNITS && rc == GSB_OK; u++) {
+    if (!(out->units >> u & 1u)) continue;
+    gsb_tensor_unit_result &ur = out->unit[u];
+    gsb_sm_args a;
+    memset(&a, 0, sizeof a);
+    a.log = reinterpret_cast<gsb_sm_log *>(base);
+    a.expected = base + offset[u];
+    a.seed = out->seed;
+    a.smem_bytes = (uint32_t)smem;
+    uint32_t covered[GSB_SM_MAX / 32] = {0};
+    // one CTA per SM: a launch that left an SM uncovered (another context held it) is repeated
+    while (ur.launches < GSB_SPARSE_MAX_LAUNCHES && popcount_bitmap(covered) < d->sm_count) {
+      const bool hook = ur.launches == 0 && corrupt[u].armed;  // test hook: the unit's first launch only
+      a.hook_smid = hook ? corrupt[u].smid : GSB_SM_MAX;
+      a.hook_index = corrupt[u].index;
+      a.hook_xr = corrupt[u].xr;
+      ur.launches++;
+      gsb_sm_log log;
+      const int lrc = sm_launch_locked(
+          d, "sparse check",
+          [&] {
+            return chosen[u].empty() ? gsb_sparse_kernel_launch(u, d->sm_count, &a, d->stream)
+                                             : gsb_sparse_operands_launch(u, d->sm_count, &a, d->stream);
+          },
+          a.log, &log, sizeof log, 0, nullptr, &ur.kernel_ns);
+      if (lrc != GSB_OK) {
+        ur.status = rc = lrc;
+        break;
+      }
+      fold_log(log, &ur, out, covered);
+    }
+    ur.sms_covered = popcount_bitmap(covered);
+    for (int i = 0; i < GSB_SM_MAX / 32; i++) out->covered[i] = first ? covered[i] : out->covered[i] & covered[i];
+    first = false;
+  }
+  out->sms_covered = popcount_bitmap(out->covered);
+  buf.release();
+  out->wall_ns = now_ns() - t0;
+  out->status = rc;
+  bool ran = false, short_cover = false;
+  for (const gsb_tensor_unit_result &ur : out->unit) {
+    ran = ran || ur.launches != 0;
+    short_cover = short_cover || (ur.launches != 0 && ur.status == GSB_OK && ur.sms_covered < out->sm_count);
+  }
+  count_probe(d, &d->sparse.stats, *out, ran, gsb_sparse_conditions(out),
+              short_cover ? &d->sparse.stats.incomplete : nullptr);
+  return rc;
+}
+
 // ------------------------------------------------------------------ the periodic checks, described once
 
 template <typename Run>
@@ -3543,9 +3669,12 @@ using SfuCheck = Check<GSB_OPT_SFU_PROBE_EVERY_CYCLES, GSB_EVENT_SFU, &Device::s
 using L1Check = Check<GSB_OPT_L1_PROBE_EVERY_CYCLES, GSB_EVENT_L1, &Device::l1, &l1_probe_locked, &gsb_l1_conditions>;
 using OrderCheck = Check<GSB_OPT_ORDER_PROBE_EVERY_CYCLES, GSB_EVENT_ORDER, &Device::order, &order_probe_locked,
                          &gsb_order_conditions>;
+using SparseCheck = Check<GSB_OPT_SPARSE_PROBE_EVERY_CYCLES, GSB_EVENT_SPARSE, &Device::sparse, &sparse_probe_locked,
+                          &gsb_sparse_conditions>;
 // in the order the prober runs them when several are due after the same cycle; G.check_every follows it
 using Checks =
-    std::tuple<LinkCheck, CopyCheck, SmCheck, ClusterCheck, AtomicCheck, TensorCheck, SfuCheck, L1Check, OrderCheck>;
+    std::tuple<LinkCheck, CopyCheck, SmCheck, ClusterCheck, AtomicCheck, TensorCheck, SfuCheck, L1Check, OrderCheck,
+               SparseCheck>;
 static_assert(std::tuple_size<Checks>::value == std::extent<decltype(G.check_every)>::value, "one cadence per check");
 
 // f(check, its place in Checks) for every periodic check, in order
@@ -4535,6 +4664,69 @@ uint64_t tensor_word_mask(uint32_t unit) {
 }  // namespace
 
 extern "C" {
+
+int gsb_sparse_probe(uint32_t idx, const gsb_sparse_cfg *cfg, gsb_sparse_result *out) {
+  return probe_entry(idx, cfg, out, &SparseCheck::run);
+}
+
+int gsb_sparse_stats_get(uint32_t idx, gsb_sparse_stats *out) {
+  return stats_entry(idx, out, [](Device *d) { return &d->sparse.stats; });
+}
+
+int gsb_test_sparse_corrupt(uint32_t idx, uint32_t smid, uint32_t unit, uint32_t index, uint64_t xr) {
+  std::shared_lock<std::shared_mutex> api_lk(G.api_mu);
+  if (unit >= GSB_SPARSE_UNITS || smid >= GSB_SM_MAX || index >= GSB_SPARSE_WORDS || (xr >> 32))
+    return GSB_ERR_INVALID_ARGUMENT;
+  Device *d = device_at(idx);
+  if (!d) return G.inited ? GSB_ERR_NO_DEVICE : GSB_ERR_NOT_INITIALIZED;
+  std::lock_guard<std::mutex> lk(d->smu);
+  Device::SmCorrupt &c = d->sparse.hooks.corrupt[unit];
+  c.armed = true;
+  c.smid = smid;
+  c.index = index;
+  c.xr = xr;
+  return GSB_OK;
+}
+
+int gsb_test_sparse_operands(uint32_t idx, uint32_t unit, const int32_t *a, const uint8_t *pattern, const int32_t *b,
+                             const int32_t *sa, const int32_t *sb, const uint64_t *expected) {
+  std::shared_lock<std::shared_mutex> api_lk(G.api_mu);
+  if (unit >= GSB_SPARSE_UNITS) return GSB_ERR_INVALID_ARGUMENT;
+  const gsb_sm_tensor_shape s = gsb_sparse_shape(unit);
+  const uint32_t K = s.k, groups = gsb_sparse_groups(unit);
+  // S8: the full int8 range; otherwise [-amp, amp], as the generator makes them
+  const int32_t a_lo = unit == GSB_SPARSE_UNIT_S8_SP ? -128 : -s.amp_a, a_hi = unit == GSB_SPARSE_UNIT_S8_SP ? 127 : s.amp_a;
+  const int32_t b_lo = unit == GSB_SPARSE_UNIT_S8_SP ? -128 : -s.amp_b, b_hi = unit == GSB_SPARSE_UNIT_S8_SP ? 127 : s.amp_b;
+  std::vector<uint32_t> t;
+  if (a) {
+    if (!pattern || !b || !sa || !sb || !expected) return GSB_ERR_INVALID_ARGUMENT;
+    for (uint32_t n = 0; n < GSB_SM_M * K / 2; n++)
+      if (a[n] < a_lo || a[n] > a_hi) return GSB_ERR_INVALID_ARGUMENT;
+    for (uint32_t n = 0; n < GSB_SM_M * groups; n++)
+      if (pattern[n] >= gsb_sparse_patterns(unit)) return GSB_ERR_INVALID_ARGUMENT;
+    for (uint32_t n = 0; n < K * GSB_SM_N; n++)
+      if (b[n] < b_lo || b[n] > b_hi) return GSB_ERR_INVALID_ARGUMENT;
+    for (uint32_t i = 0; i < GSB_SM_M; i++)
+      if (sa[i] < s.sa_min || sa[i] > s.sa_max) return GSB_ERR_INVALID_ARGUMENT;
+    for (uint32_t j = 0; j < GSB_SM_N; j++)
+      if (sb[j] < s.sb_min || sb[j] > s.sb_max) return GSB_ERR_INVALID_ARGUMENT;
+    for (uint32_t w = 0; w < GSB_SPARSE_WORDS; w++)
+      if (expected[w] >> 32) return GSB_ERR_INVALID_ARGUMENT;
+    t.resize(GSB_SPARSE_WORDS + gsb_sparse_table_words(unit));
+    for (uint32_t w = 0; w < GSB_SPARSE_WORDS; w++) t[w] = (uint32_t)expected[w];
+    uint32_t *tab = t.data() + GSB_SPARSE_WORDS;
+    memcpy(tab + gsb_sparse_table_a(unit, 0, 0), a, GSB_SM_M * K / 2 * sizeof(int32_t));
+    for (uint32_t n = 0; n < GSB_SM_M * groups; n++) tab[gsb_sparse_table_p(unit, 0, 0) + n] = pattern[n];
+    memcpy(tab + gsb_sparse_table_b(unit, 0, 0), b, K * GSB_SM_N * sizeof(int32_t));
+    memcpy(tab + gsb_sparse_table_sa(unit, 0), sa, GSB_SM_M * sizeof(int32_t));
+    memcpy(tab + gsb_sparse_table_sb(unit, 0), sb, GSB_SM_N * sizeof(int32_t));
+  }
+  Device *d = device_at(idx);
+  if (!d) return G.inited ? GSB_ERR_NO_DEVICE : GSB_ERR_NOT_INITIALIZED;
+  std::lock_guard<std::mutex> lk(d->smu);
+  d->sparse.hooks.operands[unit].swap(t);
+  return GSB_OK;
+}
 
 int gsb_test_tensor_corrupt(uint32_t idx, uint32_t smid, uint32_t unit, uint32_t index, uint64_t xr) {
   std::shared_lock<std::shared_mutex> api_lk(G.api_mu);

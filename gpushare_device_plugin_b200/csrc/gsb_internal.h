@@ -165,6 +165,18 @@ int gsb_tensor_operands_launch(uint32_t unit, uint32_t grid, const gsb_sm_args *
 int gsb_tensor_kernel_preload(int smem_bytes);
 int gsb_tensor_operands_preload(int smem_bytes);
 
+/* Enqueue one sparse tensor-core check launch (sparse_check_sm90a.cu, libgpushare_b200_sparse.so) of
+ * GSB_SPARSE_UNIT_* `unit` with `grid` CTAs on `stream`. Its log and arguments are the SM check's: gsb_sm_log, and
+ * gsb_sm_args whose `expected` holds the 8192 D words (uint32 each). Returns cudaError_t as int. */
+int gsb_sparse_kernel_launch(uint32_t unit, uint32_t grid, const gsb_sm_args *a, cudaStream_t stream);
+/* The same for a unit's test-only twin (sparse_operands_sm90a.cu, gsb_test_sparse_operands): its operands and patterns
+ * are the table after the 8192 expected words (gsb_sparse_table_* in gsb_sparse_kat.h). */
+int gsb_sparse_operands_launch(uint32_t unit, uint32_t grid, const gsb_sm_args *a, cudaStream_t stream);
+/* Load the sparse check's kernels (and, for the second, their twins) into the CURRENT context and let each take
+ * `smem_bytes` of dynamic shared memory. */
+int gsb_sparse_kernel_preload(int smem_bytes);
+int gsb_sparse_operands_preload(int smem_bytes);
+
 /* Arguments of one SM special-function check launch (sfu_check_sm90a.cu): the SM check's, whose `expected` holds an
  * exact unit's folds (uint64, index op * 256 + thread), and for MUFU where each CTA writes its folds, raw results and
  * %smid (indexed by blockIdx; layout as gsb_sfu_vote reads them). */

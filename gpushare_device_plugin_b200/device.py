@@ -800,6 +800,84 @@ test_tensor_corrupt.__test__ = False
 test_tensor_operands.__test__ = False
 
 
+def sparse_probe(idx: int, *, seed: int = 0, seed_expect: int = 0, units: int = 0,
+                 raise_on_error: bool = True) -> "_abi.SparseResult":
+    """Sparse tensor-core probe of device `idx`: one D per unit (`units`: a mask of 1 << GSB_SPARSE_UNIT_*, 0 = all)
+    on every SM, compared bit for bit with the answers for `seed_expect` (0 = `seed`; `seed` 0 = fresh). Mismatches
+    are a result, not an error; with raise_on_error=False a failed launch is too (``status`` < 0)."""
+    cfg = _abi.SparseCfg(seed, seed_expect, units, 0)
+    r = _abi.SparseResult()
+    rc = lib.gsb_sparse_probe(idx, C.byref(cfg), C.byref(r))
+    if raise_on_error:
+        check(rc, f"gsb_sparse_probe({idx})")
+    return r
+
+
+def sparse_stats(idx: int) -> "_abi.SparseStats":
+    """Sparse probes of device `idx` since health_start: count, faults, skipped, incomplete, the last result."""
+    st = _abi.SparseStats()
+    check(lib.gsb_sparse_stats_get(idx, C.byref(st)), f"gsb_sparse_stats_get({idx})")
+    return st
+
+
+def sparse_expected(unit: int, seed: int) -> List[int]:
+    """The 8192 D words of sparse unit `unit` for `seed`, row-major (FP32 bits, S8_SP's S32)."""
+    n = check(int(lib.gsb_sparse_expected(unit, seed, None, 0)), "gsb_sparse_expected(size)")
+    out = (C.c_uint32 * n)()
+    check(int(lib.gsb_sparse_expected(unit, seed, out, n)), "gsb_sparse_expected")
+    return list(out)
+
+
+def sparse_conditions(r: "_abi.SparseResult") -> int:
+    """GSB_SPARSE_* bits a sparse probe result raises."""
+    return lib.gsb_sparse_conditions(C.byref(r))
+
+
+def sparse_text(r: "_abi.SparseResult", uuid: str) -> str:
+    """The one log line both daemons print for a sparse probe result."""
+    need = lib.gsb_sparse_text(C.byref(r), uuid.encode(), None, 0)
+    check(int(need), "gsb_sparse_text(size)")
+    buf = C.create_string_buffer(int(need))
+    n = lib.gsb_sparse_text(C.byref(r), uuid.encode(), buf, int(need))
+    check(int(n), "gsb_sparse_text")
+    return buf.raw[: int(n)].decode()
+
+
+def test_sparse_corrupt(idx: int, smid: int, unit: int, index: int, xr: int) -> None:
+    """Test hook: on the next sparse probe of `idx`, the CTA on SM `smid` XORs `xr` into its D word `index` of `unit`
+    just before the compare; once."""
+    check(lib.gsb_test_sparse_corrupt(idx, smid, unit, index, xr), f"gsb_test_sparse_corrupt({idx})")
+
+
+def test_sparse_operands(idx: int, unit: int, a=None, pattern=None, b=None, sa=None, sb=None, expected=None) -> None:
+    """Test hook: the next sparse probe of `idx` that runs `unit` runs it on the compressed A'[64][K/2] `a`, its
+    patterns `pattern[64][groups]`, B'[K][128] `b` and the scales `sa[64]`, `sb[128]` (integer sequences, row-major)
+    and compares D with `expected` (8192 words, row-major, as gsb_sparse_expected gives them); once. `a` None disarms
+    it."""
+    if a is None:
+        check(lib.gsb_test_sparse_operands(idx, unit, None, None, None, None, None, None),
+              f"gsb_test_sparse_operands({idx})")
+        return
+
+    def arr(ctype, xs):
+        xs = [int(x) for x in (xs.reshape(-1) if hasattr(xs, "reshape") else xs)]
+        return (ctype * len(xs))(*xs)
+    i32 = C.c_int32
+    K = _abi.SPARSE_UNIT_K[unit]
+    groups = K // 2 if unit == _abi.GSB_SPARSE_UNIT_TF32_SP else K // 4
+    a_, p_, b_, sa_, sb_ = arr(i32, a), arr(C.c_uint8, pattern), arr(i32, b), arr(i32, sa), arr(i32, sb)
+    exp = arr(C.c_uint64, expected)
+    if (len(a_) != 64 * K // 2 or len(p_) != 64 * groups or len(b_) != K * 128 or len(sa_) != 64 or len(sb_) != 128
+            or len(exp) != 8192):
+        raise ValueError("test_sparse_operands: a is 64 x K/2, pattern 64 x groups, b K x 128, sa 64, sb 128, "
+                         "expected 8192 words")
+    check(lib.gsb_test_sparse_operands(idx, unit, a_, p_, b_, sa_, sb_, exp), f"gsb_test_sparse_operands({idx})")
+
+
+test_sparse_corrupt.__test__ = False
+test_sparse_operands.__test__ = False
+
+
 def sfu_probe(idx: int, *, seed: int = 0, seed_expect: int = 0, units: int = 0,
               raise_on_error: bool = True) -> "_abi.SfuResult":
     """SM special-function probe of device `idx`: every instruction of each unit (`units`: a mask of

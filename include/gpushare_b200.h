@@ -47,7 +47,9 @@ extern "C" {
                               likewise, found by gsb_tensor_probe; SM special-function health (gsb_sfu_*,
                               GSB_EVENT_SFU) likewise, found by gsb_sfu_probe; L1 and constant-cache health
                               (gsb_l1_*, GSB_EVENT_L1) likewise, found by gsb_l1_probe; memory-ordering health
-                              (gsb_order_*, GSB_EVENT_ORDER) likewise, found by gsb_order_probe */
+                              (gsb_order_*, GSB_EVENT_ORDER) likewise, found by gsb_order_probe; sparse
+                              tensor-core health (gsb_sparse_*, GSB_EVENT_SPARSE) likewise, found by
+                              gsb_sparse_probe */
 
 /* = NVML_DEVICE_UUID_BUFFER_SIZE (vendor/.../nvml/nvml.h:1567), used by bindings.go:20 szUUID */
 #define GSB_UUID_BUFFER_SIZE 80
@@ -172,9 +174,13 @@ enum {
                                             link, copy, SM, SM-to-SM, L2 atomic, tensor-core format and SFU probes
                                             when they are due), and raises GSB_EVENT_L1; 0 = off (default): no
                                             buffer, no launch */
-  GSB_OPT_ORDER_PROBE_EVERY_CYCLES = 16   /* N > 0: each prober thread runs gsb_order_probe after its first cycle of
+  GSB_OPT_ORDER_PROBE_EVERY_CYCLES = 16,  /* N > 0: each prober thread runs gsb_order_probe after its first cycle of
+                                            a health session and after every Nth cycle, outside gsb_cycle (after the
+                                            link to L1 probes when they are due), and raises GSB_EVENT_ORDER; 0 = off
+                                            (default): no buffer, no launch */
+  GSB_OPT_SPARSE_PROBE_EVERY_CYCLES = 17  /* N > 0: each prober thread runs gsb_sparse_probe after its first cycle of
                                             a health session and after every Nth cycle, outside gsb_cycle (after every
-                                            other periodic probe that is due), and raises GSB_EVENT_ORDER; 0 = off
+                                            other periodic probe that is due), and raises GSB_EVENT_SPARSE; 0 = off
                                             (default): no buffer, no launch */
 };
 enum {
@@ -342,8 +348,10 @@ enum {
                                   GSB_SFU_* bit */
   GSB_EVENT_L1 = 0x40000,      /* GSB_OPT_L1_PROBE_EVERY_CYCLES: an L1 or constant-cache condition; edata = one
                                   GSB_L1_* bit */
-  GSB_EVENT_ORDER = 0x80000    /* GSB_OPT_ORDER_PROBE_EVERY_CYCLES: a memory-ordering condition; edata = one
+  GSB_EVENT_ORDER = 0x80000,   /* GSB_OPT_ORDER_PROBE_EVERY_CYCLES: a memory-ordering condition; edata = one
                                   GSB_ORDER_* bit */
+  GSB_EVENT_SPARSE = 0x100000  /* GSB_OPT_SPARSE_PROBE_EVERY_CYCLES: a sparse tensor-core condition; edata = one
+                                  GSB_SPARSE_* bit */
 };
 enum { GSB_PROBE_FAULT_MISMATCH = 1, GSB_PROBE_FAULT_LAUNCH = 2, GSB_PROBE_RECOVERED = 3,
        GSB_PROBE_FAULT_WEDGED = 4 /* the launch outlived the completion watchdog */ };
@@ -1962,6 +1970,110 @@ int gsb_test_order_inject(uint32_t idx, uint32_t smid, uint32_t unit, uint32_t i
  * MP_RELACQ launch, so its consumer reads every location LOST. Refused before any device is touched when smid >=
  * GSB_SM_MAX. */
 int gsb_test_order_skip(uint32_t idx, uint32_t smid);
+
+/* ---- Sparse tensor-core health (not in the reference; opt-in: GSB_OPT_SPARSE_PROBE_EVERY_CYCLES) ---------------- */
+
+/*
+ * Known-answer checks of the 2:4-sparse tensor-core forms (1:2 for TF32), on every SM. Each unit is one launch as in the
+ * tensor-core format check: one CTA per SM, each asking for the opt-in maximum of dynamic shared memory, thread 0
+ * recording %smid, a launch that left an SM uncovered repeated up to GSB_SPARSE_MAX_LAUNCHES times. Each computes one
+ * 64 x 128 D = A B, A 64 x K stored compressed (K / 2 values per row) with its metadata, and compares every word bit
+ * for bit, on the SM, with answers computed exactly on the host (gsb_sparse_expected). K is the logical K:
+ *
+ *   F16_SP     wgmma.sp m64n128k32 .f32.f16.f16, K = 512
+ *   BF16_SP    wgmma.sp m64n128k32 .f32.bf16.bf16, K = 512
+ *   TF32_SP    wgmma.sp m64n128k16 .f32.tf32.tf32, K = 256 (1:2)
+ *   E4M3_SP    wgmma.sp m64n128k64 .f32.e4m3.e4m3, K = 128
+ *   E5M2_SP    wgmma.sp m64n128k64 .f32.e5m2.e5m2, K = 128
+ *   S8_SP      wgmma.sp m64n128k64 .s32.s8.s8, K = 512
+ *   HMMA_SP    mma.sp::ordered_metadata m16n8k32 .f32.f16.f16.f32, fragments loaded with ldmatrix, K = 512
+ *
+ * Every (row, group of four K) keeps one of the six increasing index pairs, drawn from the seed (TF32: one of each
+ * pair of K). The 16-bit and TF32 units alternate sparsity selector 0 and 1 over their K steps, so both thread pairs'
+ * metadata are read. HMMA_SP runs F16_SP's operands, so its answer is F16_SP's. The operands are generated on the
+ * device from (unit, seed, row, col); only the expected answers are uploaded, into a transient buffer taken only when
+ * GSB_OPT_TRANSIENT_KEEP_FREE_BYTES stays free. A mismatch never touches the HBM fault log or reports.
+ */
+enum {
+  GSB_SPARSE_UNIT_F16_SP = 0,
+  GSB_SPARSE_UNIT_BF16_SP = 1,
+  GSB_SPARSE_UNIT_TF32_SP = 2,
+  GSB_SPARSE_UNIT_E4M3_SP = 3,
+  GSB_SPARSE_UNIT_E5M2_SP = 4,
+  GSB_SPARSE_UNIT_S8_SP = 5,
+  GSB_SPARSE_UNIT_HMMA_SP = 6
+};
+#define GSB_SPARSE_UNITS 7
+#define GSB_SPARSE_RECORDS 64
+#define GSB_SPARSE_MAX_LAUNCHES 3
+#define GSB_SPARSE_WORDS 8192 /* D words of one CTA: 64 x 128 */
+
+typedef struct gsb_sparse_cfg {
+  uint32_t seed;        /* operands' seed; 0 = fresh per probe */
+  uint32_t seed_expect; /* seed of the expected answers; 0 = seed */
+  uint32_t units;       /* mask of 1 << GSB_SPARSE_UNIT_*; 0 = all */
+  uint32_t reserved0;
+} gsb_sparse_cfg;
+
+/* per unit: gsb_tensor_unit_result, its fields meaning the same */
+typedef struct gsb_sparse_result {
+  int32_t status;          /* GSB_OK iff every unit asked for ran every launch (mismatches are a result) */
+  uint32_t sm_count;       /* the device's multiProcessorCount = the grid of every launch */
+  uint32_t seed, seed_expect, units;
+  uint32_t sms_covered;    /* SMs covered by every unit that ran */
+  uint32_t covered[GSB_SM_MAX / 32];  /* their bitmap, bit smid */
+  uint32_t faulty[GSB_SM_MAX / 32];   /* SMs with at least one wrong word */
+  gsb_tensor_unit_result unit[GSB_SPARSE_UNITS];
+  uint32_t n_records;      /* records filled (the first GSB_SPARSE_RECORDS mismatches) */
+  uint32_t reserved0;
+  /* unit: GSB_SPARSE_UNIT_*; index: row * 128 + column of D; expected and observed: FP32 (S8_SP: S32) bits */
+  gsb_sm_record records[GSB_SPARSE_RECORDS];
+  uint64_t expected_ns;    /* host time spent computing the expected answers */
+  uint64_t wall_ns;        /* host time of the whole call */
+} gsb_sparse_result;
+
+/* Conditions (gsb_sparse_conditions), from the units that ran only. Coverage short of sm_count after the relaunches is
+ * counted (gsb_sparse_stats.incomplete) and logged, never a condition. */
+enum {
+  GSB_SPARSE_CORRUPT = 1u, /* a D word differs from its exact answer on some SM */
+  GSB_SPARSE_FAILED = 2u   /* a launch failed or outlived the watchdog */
+};
+
+/* Sparse probes of one device since gsb_health_start (counters restart with it; gsb_sparse_probe calls count too). */
+typedef struct gsb_sparse_stats {
+  uint64_t probes;     /* sparse probes run */
+  uint64_t faults;     /* of which raised at least one GSB_SPARSE_* condition */
+  uint64_t skipped;    /* probes that ran no unit (buffers not allocatable): no condition, no event */
+  uint64_t incomplete; /* probes in which some unit covered fewer than sm_count SMs */
+  gsb_sparse_result last;
+} gsb_sparse_stats;
+
+/* Holds the device while it runs; each launch under the completion watchdog. A probe that cannot take its buffer
+ * returns GSB_ERR_OUT_OF_MEMORY and counts as skipped. */
+int gsb_sparse_probe(uint32_t idx, const gsb_sparse_cfg *cfg, gsb_sparse_result *out);
+int gsb_sparse_stats_get(uint32_t idx, gsb_sparse_stats *out);
+/* Pure: the exact answers of `unit` for `seed`: the 8192 words of D in row-major order (FP32 bits, S8_SP's S32).
+ * Returns the count, or with out == NULL the count required, or a negative status (GSB_ERR_BUFFER_TOO_SMALL when cap is
+ * short, GSB_ERR_INVALID_ARGUMENT for an unknown unit). */
+int64_t gsb_sparse_expected(uint32_t unit, uint32_t seed, uint32_t *out, size_t cap);
+/* Pure: GSB_SPARSE_* bits that hold for a result (see above). */
+uint32_t gsb_sparse_conditions(const gsb_sparse_result *r);
+/* Pure: the one-line text both daemons log for a result. uuid may be NULL. Returns like gsb_sm_text. */
+int64_t gsb_sparse_text(const gsb_sparse_result *r, const char *uuid, char *buf, size_t cap);
+/* test hook: on the next gsb_sparse_probe of device idx, the CTA running on SM `smid` XORs xr into its D word `index`
+ * of `unit` just before the compare; once. Refused before any device is touched: unit, smid or index out of range, or
+ * xr wider than 32 bits. */
+int gsb_test_sparse_corrupt(uint32_t idx, uint32_t smid, uint32_t unit, uint32_t index, uint64_t xr);
+/* test hook: the next gsb_sparse_probe of device idx that runs `unit` runs it on chosen operands instead of the seed's:
+ * every launch of the unit in that probe computes D = A B, A[i] being row i of the compressed
+ * a[i * K / 2 + c] * 2^sa[i] spread by pattern[i * G + q] (G = K / 4 groups of four, pattern 0-5 the index pairs
+ * (0,1) (0,2) (0,3) (1,2) (1,3) (2,3); TF32_SP: G = K / 2 groups of two, pattern 0 or 1 the element kept), and
+ * B[k][j] = b[k * 128 + j] * 2^sb[j], through the same conversion, layout, metadata, instruction and compare, and
+ * compares D with expected[row * 128 + col] (as gsb_sparse_expected gives them). Once. a == NULL disarms it. Refused
+ * with GSB_ERR_INVALID_ARGUMENT before any device is touched: an unknown unit, an integer outside the unit's range, a
+ * scale outside its range, a pattern outside the unit's set, or an expected word wider than 32 bits. */
+int gsb_test_sparse_operands(uint32_t idx, uint32_t unit, const int32_t *a, const uint8_t *pattern, const int32_t *b,
+                             const int32_t *sa, const int32_t *sb, const uint64_t *expected);
 
 /* ---- Allocate (a12, a13): wire bytes in, wire bytes out ---------------------------------- */
 

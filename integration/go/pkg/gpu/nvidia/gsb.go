@@ -100,6 +100,7 @@ const (
 	gsbEventSFU       = uint64(C.GSB_EVENT_SFU)       // opt-in SM special-function health: Edata = one of the gsbSFU* conditions below
 	gsbEventL1        = uint64(C.GSB_EVENT_L1)        // opt-in L1 and constant-cache health: Edata = one of the gsbL1* conditions below
 	gsbEventOrder     = uint64(C.GSB_EVENT_ORDER)     // opt-in memory-ordering health: Edata = one of the gsbOrder* conditions below
+	gsbEventSparse    = uint64(C.GSB_EVENT_SPARSE)    // opt-in sparse tensor-core health: Edata = one of the gsbSparse* conditions below
 )
 
 const (
@@ -151,6 +152,8 @@ const (
 	gsbOrderLost      = uint64(C.GSB_ORDER_LOST)      // a store not visible after the grid barrier
 	gsbOrderTimeout   = uint64(C.GSB_ORDER_TIMEOUT)   // a grid barrier ran out: an SM stalled or a store never became visible
 	gsbOrderFailed    = uint64(C.GSB_ORDER_FAILED)    // a memory-ordering launch failed or outlived the watchdog
+	gsbSparseCorrupt  = uint64(C.GSB_SPARSE_CORRUPT)  // a sparse tensor-core D word differs from its exact answer on some SM
+	gsbSparseFailed   = uint64(C.GSB_SPARSE_FAILED)   // a sparse tensor-core launch failed or outlived the watchdog
 )
 
 const (
@@ -646,6 +649,34 @@ func gsbOrderLine(idx uint, uuid string) string {
 	}
 	buf := make([]byte, int(need))
 	n := C.gsb_order_text(&st.last, cu, (*C.char)(unsafe.Pointer(&buf[0])), C.size_t(len(buf)))
+	if n < 0 {
+		return ""
+	}
+	return string(buf[:int(n)])
+}
+
+// gsbEnableSparseHealth turns on sparse tensor-core health: each prober runs gsb_sparse_probe after its first cycle
+// of a session and after every `every`-th cycle. Call it before gsbHealthStart.
+func gsbEnableSparseHealth(every uint64) error {
+	return gsbErr(C.gsb_set_option(C.GSB_OPT_SPARSE_PROBE_EVERY_CYCLES, C.uint64_t(every)))
+}
+
+// gsbSparseLine is the one log line of GPU idx's most recent sparse tensor-core probe ("not run" when there is none):
+// what a plugin logs before marking a GPU unhealthy on a GSB_EVENT_SPARSE event.
+func gsbSparseLine(idx uint, uuid string) string {
+	st := (*C.gsb_sparse_stats)(C.calloc(1, C.size_t(unsafe.Sizeof(C.gsb_sparse_stats{}))))
+	defer C.free(unsafe.Pointer(st))
+	if C.gsb_sparse_stats_get(C.uint32_t(idx), st) != C.GSB_OK {
+		*st = C.gsb_sparse_stats{}
+	}
+	cu := C.CString(uuid)
+	defer C.free(unsafe.Pointer(cu))
+	need := C.gsb_sparse_text(&st.last, cu, nil, 0)
+	if need <= 0 {
+		return ""
+	}
+	buf := make([]byte, int(need))
+	n := C.gsb_sparse_text(&st.last, cu, (*C.char)(unsafe.Pointer(&buf[0])), C.size_t(len(buf)))
 	if n < 0 {
 		return ""
 	}
