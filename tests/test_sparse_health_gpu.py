@@ -1,4 +1,5 @@
-"""Sparse tensor-core health on a real H100. First the layout-pinning cases through chosen operands, exact on every SM:
+"""Sparse tensor-core health on a real H100. First the layout-pinning cases (tests/helpers/sparse_edges.py; the other
+chosen cases are tests/test_sparse_edges_gpu.py's) through chosen operands, exact on every SM:
 each pattern alone, one pattern per row, patterns rotating per group, one-hot A' against a B whose rows encode their
 own index, the largest kept sum the operand ranges allow with alternating signs, and a flipped expected bit caught
 once per SM. Then a clean default probe and each unit alone, a wrong seed_expect (exact counts and records), the
@@ -10,11 +11,11 @@ import subprocess
 import sys
 import time
 
-import numpy as np
 import pytest
 
 from gpushare_device_plugin_b200 import _abi
 from tests.helpers import sparse_oracle as so
+from tests.helpers.sparse_edges import layout_cases
 
 pytestmark = pytest.mark.gpu
 
@@ -56,53 +57,6 @@ def assert_clean(gsb, r, units=tuple(UNITS)):
 
 
 # ---------------------------------------------------------------- layout-pinning cases (chosen operands)
-
-def amps(unit):
-    _, amp_a, amp_b = so.SHAPES[unit][:3]
-    if unit == so.S8_SP:
-        return 127, 127
-    return amp_a, amp_b
-
-
-def layout_cases(unit):
-    """(name, A', P, B', sa, sb) whose D pins the metadata layout. Row k of B holds (k + j) mod (2 amp_b + 1) - amp_b
-    in column j: the four rows of every group differ in every column (2 amp_b + 1 >= 7), so a stored value that
-    meets the wrong row of its group gives a wrong word, and a wrong word names the row it took modulo 2 amp_b + 1
-    (255 for F16, BF16 and HMMA_SP, 127 for TF32, 255 for S8, but only 7 for E4M3 and 15 for E5M2).
-
-    The largest kept sum the operand ranges allow is K/2 amp_a amp_b: for the FP8 units 64 x 15 x 3 = 2 880 (E4M3) and
-    64 x 7 x 7 = 3 136 (E5M2). The FP8 bound of 2^12 - 1 itself cannot be reached through gsb_test_sparse_operands,
-    which takes only the integers the generator can make."""
-    K = so.SHAPES[unit][0]
-    groups = K // so.group(unit)
-    rng = np.random.default_rng(1000 + unit)
-    amp_a, amp_b = amps(unit)
-    za, zb = np.zeros(so.M, np.int64), np.zeros(so.N, np.int64)
-    small_a = rng.integers(-amp_a, amp_a + 1, size=(so.M, K // 2))
-    # B whose row k holds k mod (2 amp_b + 1) - amp_b, offset by column: D words differ per kept row
-    enc_b = (np.arange(K)[:, None] + np.arange(so.N)[None, :]) % (2 * amp_b + 1) - amp_b
-    out = []
-    for p in range(so.n_patterns(unit)):
-        out.append((f"pattern{p}", small_a, np.full((so.M, groups), p), enc_b, za, zb))
-    out.append(("pattern_per_row", small_a, np.repeat((np.arange(so.M) % so.n_patterns(unit))[:, None], groups, 1),
-                enc_b, za, zb))
-    out.append(("pattern_rotating", small_a,
-                (np.arange(so.M)[:, None] + np.arange(groups)[None, :]) % so.n_patterns(unit), enc_b, za, zb))
-    # one-hot A': row i keeps one nonzero stored value, at stored column c(i); the rest zero
-    onehot = np.zeros((so.M, K // 2), np.int64)
-    cols = (np.arange(so.M) * 7) % (K // 2)
-    onehot[np.arange(so.M), cols] = 1
-    rand_p = rng.integers(0, so.n_patterns(unit), size=(so.M, groups))
-    out.append(("onehot", onehot, rand_p, enc_b, za, zb))
-    # the largest kept sum the ranges allow: |A'| amp_a, |B'| amp_b on every kept term, signs alternating by row and column
-    K2 = K // 2
-    lim = so.SHAPES[unit][5]
-    if K2 * amp_a * amp_b < lim:
-        sgn_a = np.where(np.arange(so.M)[:, None] % 2 == 0, 1, -1) * np.ones((1, K2), np.int64)
-        sgn_b = np.where(np.arange(so.N)[None, :] % 2 == 0, 1, -1) * np.ones((K, 1), np.int64)
-        out.append(("bound_signs", amp_a * sgn_a, rand_p, amp_b * sgn_b, za, zb))
-    return out
-
 
 def run_case(gsb, unit, A, P, B, sa, sb, flip=None):
     want = so.gemm_from(unit, A, P, B, sa, sb)
