@@ -24,6 +24,7 @@ $NVCC $FLAGS -Xptxas -v -c $SRC/sfu_operands_sm90a.cu -o build/sfu_operands_sm90
 $NVCC $FLAGS -Xptxas -v -c $SRC/order_check_sm90a.cu -o build/order_check_sm90a.o 2> build/ptxas_order_check.log || { cat build/ptxas_order_check.log; exit 1; }
 $NVCC $FLAGS -Xptxas -v -c $SRC/sparse_check_sm90a.cu -o build/sparse_check_sm90a.o 2> build/ptxas_sparse_check.log || { cat build/ptxas_sparse_check.log; exit 1; }
 $NVCC $FLAGS -Xptxas -v -c $SRC/sparse_operands_sm90a.cu -o build/sparse_operands_sm90a.o 2> build/ptxas_sparse_operands.log || { cat build/ptxas_sparse_operands.log; exit 1; }
+$NVCC $FLAGS -Xptxas -v -c $SRC/shared_atomic_check_sm90a.cu -o build/shared_atomic_check_sm90a.o 2> build/ptxas_shared_atomic_check.log || { cat build/ptxas_shared_atomic_check.log; exit 1; }
 $NVCC $FLAGS -Xptxas -v -c $SRC/l1_check_sm90a.cu -o build/l1_check_sm90a.o 2> build/ptxas_l1_check.log || { cat build/ptxas_l1_check.log; exit 1; }
 $NVCC $FLAGS -Xptxas -v -c $SRC/l1_table_sm90a.cu -o build/l1_table_sm90a.o 2> build/ptxas_l1_table.log || { cat build/ptxas_l1_table.log; exit 1; }
 # the L1 and constant-cache check's kernels are a module of their own: its 64 KiB __constant__ bank fills the whole user
@@ -39,6 +40,8 @@ $NVCC -shared -gencode arch=compute_90a,code=sm_90a -cudart static -o $PKG/libgp
 # the sparse tensor-core check's kernels and their test-only twins likewise: a module of their own, so the recorded
 # kernel sets of the other libraries stay as they are
 $NVCC -shared -gencode arch=compute_90a,code=sm_90a -cudart static -o $PKG/libgpushare_b200_sparse.so build/sparse_check_sm90a.o build/sparse_operands_sm90a.o
+# the shared-memory atomic check's kernels likewise
+$NVCC -shared -gencode arch=compute_90a,code=sm_90a -cudart static -o $PKG/libgpushare_b200_shared_atomic.so build/shared_atomic_check_sm90a.o
 $NVCC $FLAGS -c $SRC/gsb_device.cu -o build/gsb_device.o
 g++ -O2 -std=c++17 -fPIC -Wall -c $SRC/gsb_wire.cc -o build/gsb_wire.o
 g++ -O2 -std=c++17 -fPIC -Wall -c $SRC/gsb_fault.cc -o build/gsb_fault.o
@@ -55,7 +58,8 @@ g++ -O2 -std=c++17 -fPIC -Wall -c $SRC/gsb_sfu.cc -o build/gsb_sfu.o
 g++ -O2 -std=c++17 -fPIC -Wall -c $SRC/gsb_l1.cc -o build/gsb_l1.o
 g++ -O2 -std=c++17 -fPIC -Wall -c $SRC/gsb_order.cc -o build/gsb_order.o
 g++ -O2 -std=c++17 -fPIC -Wall -c $SRC/gsb_sparse.cc -o build/gsb_sparse.o
-$NVCC -shared -gencode arch=compute_90a,code=sm_90a -cudart static -o $OUT build/hbm_probe_sm90a.o build/sm_check_sm90a.o build/mma_operands_sm90a.o build/sm_stress_sm90a.o build/cluster_check_sm90a.o build/atomic_check_sm90a.o build/atomic_values_sm90a.o build/tensor_check_sm90a.o build/tensor_operands_sm90a.o build/sfu_check_sm90a.o build/sfu_operands_sm90a.o build/gsb_device.o build/gsb_wire.o build/gsb_fault.o build/gsb_ecc.o build/gsb_memtest.o build/gsb_link.o build/gsb_copy.o build/gsb_sm.o build/gsb_stress.o build/gsb_cluster.o build/gsb_atomic.o build/gsb_tensor.o build/gsb_sfu.o build/gsb_l1.o build/gsb_order.o build/gsb_sparse.o -L$PKG -lgpushare_b200_l1 -lgpushare_b200_order -lgpushare_b200_cluster_script -lgpushare_b200_sparse -Xlinker -rpath,'$ORIGIN' -ldl -lpthread -lrt
+g++ -O2 -std=c++17 -fPIC -Wall -c $SRC/gsb_shared_atomic.cc -o build/gsb_shared_atomic.o
+$NVCC -shared -gencode arch=compute_90a,code=sm_90a -cudart static -o $OUT build/hbm_probe_sm90a.o build/sm_check_sm90a.o build/mma_operands_sm90a.o build/sm_stress_sm90a.o build/cluster_check_sm90a.o build/atomic_check_sm90a.o build/atomic_values_sm90a.o build/tensor_check_sm90a.o build/tensor_operands_sm90a.o build/sfu_check_sm90a.o build/sfu_operands_sm90a.o build/gsb_device.o build/gsb_wire.o build/gsb_fault.o build/gsb_ecc.o build/gsb_memtest.o build/gsb_link.o build/gsb_copy.o build/gsb_sm.o build/gsb_stress.o build/gsb_cluster.o build/gsb_atomic.o build/gsb_tensor.o build/gsb_sfu.o build/gsb_l1.o build/gsb_order.o build/gsb_sparse.o build/gsb_shared_atomic.o -L$PKG -lgpushare_b200_l1 -lgpushare_b200_order -lgpushare_b200_cluster_script -lgpushare_b200_sparse -lgpushare_b200_shared_atomic -Xlinker -rpath,'$ORIGIN' -ldl -lpthread -lrt
 echo "built $OUT"
 # native daemon (C++ host side: HTTP/2 + HPACK gRPC front end, kube client, manager loop) + its h2 self-test
 g++ -O2 -std=c++17 -Wall -pthread -o $PKG/gsbd $SRC/daemon/gsbd.cc -L$PKG -lgpushare_b200 -lssl -lcrypto -ldl -Wl,-rpath,'$ORIGIN'

@@ -94,6 +94,14 @@ SPARSE_UNIT_K = [512, 512, 256, 128, 128, 512, 512]  # logical K of each unit (=
 GSB_SPARSE_UNITS, GSB_SPARSE_RECORDS, GSB_SPARSE_MAX_LAUNCHES, GSB_SPARSE_WORDS = 7, 64, 3, 8192
 GSB_SPARSE_CORRUPT, GSB_SPARSE_FAILED = 1, 2
 SPARSE_CONDITION_NAMES = {1: "wrong sparse tensor-core result", 2: "sparse probe failed"}
+GSB_SHARED_ATOMIC_UNIT_INT32, GSB_SHARED_ATOMIC_UNIT_WIDE, GSB_SHARED_ATOMIC_UNIT_FLOAT, GSB_SHARED_ATOMIC_UNIT_TICKET, \
+    GSB_SHARED_ATOMIC_UNIT_CAS, GSB_SHARED_ATOMIC_UNIT_DSMEM, GSB_SHARED_ATOMIC_UNIT_REDAS = range(7)
+SHARED_ATOMIC_UNIT_NAMES = ["int32", "wide", "float", "ticket", "cas", "dsmem", "redas"]
+GSB_SHARED_ATOMIC_UNITS, GSB_SHARED_ATOMIC_RECORDS, GSB_SHARED_ATOMIC_MAX_LAUNCHES = 7, 64, 3
+GSB_SHARED_ATOMIC_AREA_WORDS, GSB_SHARED_ATOMIC_CAS_WAIT_NS, GSB_SHARED_ATOMIC_NO_SM = 3072, 100_000_000, 0xFFFFFFFF
+GSB_SHARED_ATOMIC_REC_WORD, GSB_SHARED_ATOMIC_REC_SLOT, GSB_SHARED_ATOMIC_REC_TICKET, GSB_SHARED_ATOMIC_REC_TORN = range(4)
+GSB_SHARED_ATOMIC_CORRUPT, GSB_SHARED_ATOMIC_FAILED = 1, 2
+SHARED_ATOMIC_CONDITION_NAMES = {1: "wrong shared-memory atomic result", 2: "shared-memory atomic probe failed"}
 GSB_SFU_UNIT_CVT_HALF, GSB_SFU_UNIT_CVT_FP8, GSB_SFU_UNIT_CVT_INT, GSB_SFU_UNIT_DIVSQRT, GSB_SFU_UNIT_WARP, \
     GSB_SFU_UNIT_MUFU = range(6)
 SFU_UNIT_NAMES = ["cvt_half", "cvt_fp8", "cvt_int", "divsqrt", "warp", "mufu"]
@@ -146,8 +154,8 @@ VARIANT_NAMES = {0: "auto", 1: "direct", 2: "cpasync", 3: "bulk", 4: "bulkw", 5:
 GSB_PROBE_TIMED, GSB_PROBE_SEED_TABLE = 1, 2
 GSB_EVENT_XID, GSB_EVENT_PROBE, GSB_EVENT_INVENTORY, GSB_EVENT_ECC, GSB_EVENT_LINK, GSB_EVENT_COPY, GSB_EVENT_SM, \
     GSB_EVENT_CLUSTER, GSB_EVENT_ATOMIC, GSB_EVENT_TENSOR, GSB_EVENT_SFU, GSB_EVENT_L1, GSB_EVENT_ORDER, \
-    GSB_EVENT_SPARSE = 8, 0x100, 0x200, 0x400, 0x800, 0x1000, 0x2000, 0x4000, 0x8000, 0x10000, 0x20000, 0x40000, \
-    0x80000, 0x100000
+    GSB_EVENT_SPARSE, GSB_EVENT_SHARED_ATOMIC = 8, 0x100, 0x200, 0x400, 0x800, 0x1000, 0x2000, 0x4000, 0x8000, \
+    0x10000, 0x20000, 0x40000, 0x80000, 0x100000, 0x200000
 GSB_PROBE_FAULT_MISMATCH, GSB_PROBE_FAULT_LAUNCH, GSB_PROBE_RECOVERED, GSB_PROBE_FAULT_WEDGED = 1, 2, 3, 4
 GSB_INVENTORY_IDENTITY_CHANGED, GSB_INVENTORY_TOTAL_CHANGED = 1, 2
 GSB_ECC_VALID_MODE, GSB_ECC_VALID_VOLATILE, GSB_ECC_VALID_AGGREGATE, GSB_ECC_VALID_DRAM, GSB_ECC_VALID_REMAP, \
@@ -166,8 +174,8 @@ GSB_OPT_INVENTORY_POLICY, GSB_OPT_WAIT_SPIN_US, GSB_OPT_WATCHDOG_MS, GSB_OPT_INV
     GSB_OPT_TRANSIENT_KEEP_FREE_BYTES, GSB_OPT_SWEEP_EVERY_CYCLES, GSB_OPT_ECC_HEALTH, GSB_OPT_LINK_PROBE_EVERY_CYCLES, \
     GSB_OPT_COPY_PROBE_EVERY_CYCLES, GSB_OPT_SM_PROBE_EVERY_CYCLES, GSB_OPT_CLUSTER_PROBE_EVERY_CYCLES, \
     GSB_OPT_ATOMIC_PROBE_EVERY_CYCLES, GSB_OPT_TENSOR_PROBE_EVERY_CYCLES, GSB_OPT_SFU_PROBE_EVERY_CYCLES, \
-    GSB_OPT_L1_PROBE_EVERY_CYCLES, GSB_OPT_ORDER_PROBE_EVERY_CYCLES, GSB_OPT_SPARSE_PROBE_EVERY_CYCLES = \
-    1, 2, 3, 4, 5, 6, 7, 8, 9, 10, 11, 12, 13, 14, 15, 16, 17
+    GSB_OPT_L1_PROBE_EVERY_CYCLES, GSB_OPT_ORDER_PROBE_EVERY_CYCLES, GSB_OPT_SPARSE_PROBE_EVERY_CYCLES, \
+    GSB_OPT_SHARED_ATOMIC_PROBE_EVERY_CYCLES = 1, 2, 3, 4, 5, 6, 7, 8, 9, 10, 11, 12, 13, 14, 15, 16, 17, 18
 GSB_INVENTORY_SNAPSHOT, GSB_INVENTORY_LIVE = 0, 1
 GSB_ALLOC_MATCHED, GSB_ALLOC_SINGLE_GPU, GSB_ALLOC_ERR_RESPONSE = 1, 2, 3
 UINT64_MAX = (1 << 64) - 1
@@ -205,6 +213,9 @@ SYMBOLS = [
     "gsb_order_classify", "gsb_order_conditions", "gsb_order_text", "gsb_test_order_inject", "gsb_test_order_skip",
     "gsb_sparse_probe", "gsb_sparse_stats_get", "gsb_sparse_expected", "gsb_sparse_conditions", "gsb_sparse_text",
     "gsb_test_sparse_corrupt", "gsb_test_sparse_operands",
+    "gsb_shared_atomic_probe", "gsb_shared_atomic_stats_get", "gsb_shared_atomic_expected",
+    "gsb_shared_atomic_conditions", "gsb_shared_atomic_text", "gsb_test_shared_atomic_corrupt",
+    "gsb_test_shared_atomic_skip",
     "gsb_allocate", "gsb_allocate_err_response", "gsb_patch_assigned_body",
 ]
 
@@ -894,6 +905,75 @@ class SparseStats(C.Structure):
     ]
 
 
+class SharedAtomicCfg(C.Structure):
+    _fields_ = [
+        ("units", C.c_uint32),
+        ("seed", C.c_uint32),
+        ("seed_expect", C.c_uint32),
+        ("reserved0", C.c_uint32),
+    ]
+
+
+class SharedAtomicRecord(C.Structure):
+    _fields_ = [
+        ("smid", C.c_uint32),
+        ("unit", C.c_uint32),
+        ("kind", C.c_uint32),  # GSB_SHARED_ATOMIC_REC_*
+        ("index", C.c_uint32),
+        ("expected", C.c_uint64),
+        ("observed", C.c_uint64),
+    ]
+
+
+class SharedAtomicRun(C.Structure):
+    _fields_ = [
+        ("status", C.c_int32),
+        ("launches", C.c_uint32),
+        ("sms_covered", C.c_uint32),
+        ("hook_cta", C.c_uint32),
+        ("cluster_launches", C.c_uint32 * 2),
+        ("clusters", C.c_uint32 * 2),
+        ("atomics_issued", C.c_uint64),
+        ("words_checked", C.c_uint64),
+        ("mismatch_words", C.c_uint64),
+        ("mismatch_bits", C.c_uint64),
+        ("ticket_faults", C.c_uint64),
+        ("timeouts", C.c_uint64),
+        ("cas_max_ns", C.c_uint64),
+        ("kernel_ns", C.c_uint64),
+    ]
+
+
+class SharedAtomicResult(C.Structure):
+    _fields_ = [
+        ("status", C.c_int32),
+        ("sm_count", C.c_uint32),
+        ("seed", C.c_uint32),
+        ("seed_expect", C.c_uint32),
+        ("units", C.c_uint32),
+        ("sms_covered", C.c_uint32),
+        ("covered", C.c_uint32 * (GSB_SM_MAX // 32)),
+        ("faulty", C.c_uint32 * (GSB_SM_MAX // 32)),
+        ("cluster_n", C.c_uint32 * 2),
+        ("run", SharedAtomicRun * GSB_SHARED_ATOMIC_UNITS),
+        ("n_records", C.c_uint32),
+        ("reserved0", C.c_uint32),
+        ("records", SharedAtomicRecord * GSB_SHARED_ATOMIC_RECORDS),
+        ("expected_ns", C.c_uint64),
+        ("wall_ns", C.c_uint64),
+    ]
+
+
+class SharedAtomicStats(C.Structure):
+    _fields_ = [
+        ("probes", C.c_uint64),
+        ("faults", C.c_uint64),
+        ("skipped", C.c_uint64),
+        ("incomplete", C.c_uint64),
+        ("last", SharedAtomicResult),
+    ]
+
+
 class SfuCfg(C.Structure):
     _fields_ = [
         ("seed", C.c_uint32),
@@ -1255,6 +1335,13 @@ def _load() -> C.CDLL:
         "gsb_sparse_text": (C.c_int64, [C.POINTER(SparseResult), C.c_char_p, C.c_char_p, C.c_size_t]),
         "gsb_test_sparse_corrupt": (C.c_int, [C.c_uint32, C.c_uint32, C.c_uint32, C.c_uint32, C.c_uint64]),
         "gsb_test_sparse_operands": (C.c_int, [C.c_uint32, C.c_uint32, i32p, u8p, i32p, i32p, i32p, u64p]),
+        "gsb_shared_atomic_probe": (C.c_int, [C.c_uint32, C.POINTER(SharedAtomicCfg), C.POINTER(SharedAtomicResult)]),
+        "gsb_shared_atomic_stats_get": (C.c_int, [C.c_uint32, C.POINTER(SharedAtomicStats)]),
+        "gsb_shared_atomic_expected": (C.c_int64, [C.c_uint32, C.c_uint32, C.c_uint32, C.c_uint32, u32p, C.c_size_t]),
+        "gsb_shared_atomic_conditions": (C.c_uint32, [C.POINTER(SharedAtomicResult)]),
+        "gsb_shared_atomic_text": (C.c_int64, [C.POINTER(SharedAtomicResult), C.c_char_p, C.c_char_p, C.c_size_t]),
+        "gsb_test_shared_atomic_corrupt": (C.c_int, [C.c_uint32, C.c_uint32, C.c_uint32, C.c_uint32, C.c_uint64]),
+        "gsb_test_shared_atomic_skip": (C.c_int, [C.c_uint32, C.c_uint32, C.c_uint32]),
         "gsb_allocate": (C.c_int, [C.POINTER(AllocateCtx), C.POINTER(Pod), C.c_uint32, C.c_char_p, C.c_size_t, C.c_void_p, C.c_size_t, C.POINTER(C.c_size_t), C.POINTER(C.c_int32), u32p]),
         "gsb_allocate_err_response": (C.c_int, [C.POINTER(AllocateCtx), C.c_char_p, C.c_size_t, C.c_void_p, C.c_size_t, C.POINTER(C.c_size_t)]),
         "gsb_patch_assigned_body": (C.c_int, [C.c_uint64, C.c_char_p, C.c_size_t]),

@@ -69,6 +69,7 @@ def parse(argv):
     add("probe-l1-every", default=0, type=int)  # L1 and constant-cache probe every N prober cycles; 0 = off
     add("probe-order-every", default=0, type=int)  # memory-ordering probe every N prober cycles; 0 = off
     add("probe-sparse-every", default=0, type=int)  # sparse tensor-core probe every N prober cycles; 0 = off
+    add("probe-shared-atomic-every", default=0, type=int)  # shared-memory atomic probe every N prober cycles; 0 = off
     return p.parse_args(argv)
 
 
@@ -114,7 +115,8 @@ def main(argv=None) -> None:  # main.go:55-65
                               probe_cluster_every=a.probe_cluster_every, probe_atomic_every=a.probe_atomic_every,
                               probe_tensor_every=a.probe_tensor_every, probe_sfu_every=a.probe_sfu_every,
                               probe_l1_every=a.probe_l1_every, probe_order_every=a.probe_order_every,
-                              probe_sparse_every=a.probe_sparse_every)
+                              probe_sparse_every=a.probe_sparse_every,
+                              probe_shared_atomic_every=a.probe_shared_atomic_every)
     ngm.Run()
 
 

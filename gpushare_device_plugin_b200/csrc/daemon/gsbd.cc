@@ -182,6 +182,15 @@ const Check kChecks[] = {
      },
      {{GSB_SPARSE_CORRUPT, "wrong sparse tensor-core result"}, {GSB_SPARSE_FAILED, "sparse probe failed"}},
      "sparse condition ?"},
+    {&Flags::probe_shared_atomic_every, GSB_OPT_SHARED_ATOMIC_PROBE_EVERY_CYCLES, GSB_EVENT_SHARED_ATOMIC,
+     "shared-memory atomic health", "shared-atomic",
+     [](uint32_t i, const std::string &u) {
+       return probed<gsb_shared_atomic_stats>(i, u, gsb_shared_atomic_stats_get, gsb_shared_atomic_text, nullptr,
+                                              &gsb_shared_atomic_stats::incomplete);
+     },
+     {{GSB_SHARED_ATOMIC_CORRUPT, "wrong shared-memory atomic result"},
+      {GSB_SHARED_ATOMIC_FAILED, "shared-memory atomic probe failed"}},
+     "shared-memory atomic condition ?"},
 };
 constexpr size_t kNumChecks = sizeof kChecks / sizeof kChecks[0];
 

@@ -34,6 +34,7 @@ struct Flags {
   int probe_l1_every = 0;       // L1 and constant-cache probe every N prober cycles (GSB_OPT_L1_PROBE_EVERY_CYCLES); 0 = off
   int probe_order_every = 0;    // memory-ordering probe every N prober cycles (GSB_OPT_ORDER_PROBE_EVERY_CYCLES); 0 = off
   int probe_sparse_every = 0;   // sparse tensor-core probe every N prober cycles (GSB_OPT_SPARSE_PROBE_EVERY_CYCLES); 0 = off
+  int probe_shared_atomic_every = 0;  // shared-memory atomic probe every N prober cycles (GSB_OPT_SHARED_ATOMIC_PROBE_EVERY_CYCLES); 0 = off
   int startup_stress_ms = 0; // SM stress of every GPU for N ms before serving (gsb_sm_stress); 0 = off
   int probe_copy_every = 0;  // copy-engine probe every N prober cycles (GSB_OPT_COPY_PROBE_EVERY_CYCLES); 0 = off
   bool serialize_allocate = false;  // the reference's plugin-wide lock across the whole Allocate, PATCH included
@@ -128,6 +129,7 @@ int parse_flags(int argc, char **argv, Flags *f) {
     else if (name == "probe-l1-every") { if (!need()) return 3; f->probe_l1_every = atoi(val.c_str()); }  // likewise
     else if (name == "probe-order-every") { if (!need()) return 3; f->probe_order_every = atoi(val.c_str()); }  // likewise
     else if (name == "probe-sparse-every") { if (!need()) return 3; f->probe_sparse_every = atoi(val.c_str()); }  // likewise
+    else if (name == "probe-shared-atomic-every") { if (!need()) return 3; f->probe_shared_atomic_every = atoi(val.c_str()); }  // likewise
     else if (name == "startup-stress-ms") { if (!need()) return 3; f->startup_stress_ms = atoi(val.c_str()); }  // likewise
     else if (name == "coalesce-health") boolean(&f->coalesce_health);
     else if (name == "pod-informer") boolean(&f->pod_informer);

@@ -43,6 +43,7 @@
 #include <string>
 #include <thread>
 #include <tuple>
+#include <unordered_map>
 #include <utility>
 #include <vector>
 
@@ -55,6 +56,7 @@
 #include "gsb_l1.h"
 #include "gsb_order.h"
 #include "gsb_sparse_kat.h"
+#include "gsb_shared_atomic.h"
 
 namespace {
 
@@ -351,6 +353,12 @@ struct Device {
     std::vector<uint32_t> operands[GSB_SPARSE_UNITS];
   };
   CheckState<gsb_sparse_stats, SparseHooks> sparse;
+  // shared-memory atomic health: gsb_test_shared_atomic_corrupt and _skip, by GSB_SHARED_ATOMIC_UNIT_*
+  struct SharedAtomicHooks {
+    std::array<SmCorrupt, GSB_SHARED_ATOMIC_UNITS> corrupt;
+    std::array<SmCorrupt, GSB_SHARED_ATOMIC_UNITS> skip;  // smid only
+  };
+  CheckState<gsb_shared_atomic_stats, SharedAtomicHooks> shared_atomic;
 
   // persistent worker (gsb_cycle_all / gsb_probe_all): one host thread per device
   std::thread worker;
@@ -380,7 +388,7 @@ struct Global {
   std::atomic<uint64_t> transient_keep_free{1ull << 30};
   std::atomic<uint64_t> sweep_every{0};
   std::atomic<uint64_t> ecc_health{0};
-  std::atomic<uint64_t> check_every[10] = {};  // GSB_OPT_*_PROBE_EVERY_CYCLES, by the check's place in Checks
+  std::atomic<uint64_t> check_every[11] = {};  // GSB_OPT_*_PROBE_EVERY_CYCLES, by the check's place in Checks
 
   // one link or copy probe's pinned buffers at a time in the whole process (the DaemonSet's memory limit covers 8 GPUs)
   std::mutex link_mu;
@@ -586,6 +594,7 @@ int ensure_ready(Device *d) {
   if (pe == cudaSuccess) pe = (cudaError_t)gsb_order_kernel_preload(smem_optin);
   if (pe == cudaSuccess) pe = (cudaError_t)gsb_sparse_kernel_preload(smem_optin);
   if (pe == cudaSuccess) pe = (cudaError_t)gsb_sparse_operands_preload(smem_optin);
+  if (pe == cudaSuccess) pe = (cudaError_t)gsb_shared_atomic_kernel_preload(smem_optin);
   if (pe != cudaSuccess) {
     set_error("loading the probe kernels on %s: %s", d->uuid, cudaGetErrorString(pe));
     return (pe == cudaErrorInvalidDeviceFunction || pe == cudaErrorNoKernelImageForDevice) ? GSB_ERR_UNSUPPORTED_ARCH
@@ -3634,6 +3643,229 @@ int sparse_probe_locked(Device *d, const gsb_sparse_cfg *cfg, gsb_sparse_result 
   return rc;
 }
 
+// ------------------------------------------------------------------ shared-memory atomic health
+
+constexpr uint32_t kSharedAtomicAllUnits = (1u << GSB_SHARED_ATOMIC_UNITS) - 1;
+constexpr size_t kSharedAtomicLogBytes = (sizeof(gsb_shared_atomic_log) + 255) / 256 * 256;
+
+void shared_atomic_add_record(gsb_shared_atomic_result *out, const gsb_shared_atomic_record &rec) {
+  if (rec.smid < GSB_SM_MAX) out->faulty[rec.smid >> 5] |= 1u << (rec.smid & 31u);
+  if (out->n_records < GSB_SHARED_ATOMIC_RECORDS) out->records[out->n_records++] = rec;
+}
+
+// TICKET and CAS: per CTA, form and hot slot, the entries must name every contributor once. Add and CAS forms: entry t
+// holds the id that drew ticket t (the final counter is compared on the SM). Exchange forms: the values returned to the
+// contributors plus the final word (entry COUNT) must be the values of ids 0 .. COUNT (COUNT's is the starting word),
+// each once. Returns the entries that do not; each is recorded, naming the SM that owns the slots.
+uint64_t shared_atomic_check_slots(uint32_t unit, uint32_t seed, uint32_t ctas, const std::vector<uint32_t> &slots,
+                                   const gsb_shared_atomic_log &log, gsb_shared_atomic_result *out) {
+  constexpr uint32_t kCount = GSB_SHARED_ATOMIC_COUNT;
+  const uint32_t forms = unit == GSB_SHARED_ATOMIC_UNIT_TICKET ? 4u : 3u;
+  uint64_t bad = 0;
+  std::vector<char> seen(kCount + 1);
+  // TICKET: the id of each exchanged value, by form and hot slot, found by its first word
+  std::vector<std::unordered_map<uint32_t, uint32_t>> id_of(unit == GSB_SHARED_ATOMIC_UNIT_TICKET ? 4u * 32u : 0u);
+  for (uint32_t f = 1; f < id_of.size() / 32u; f++)
+    for (uint32_t l = 0; l < GSB_SHARED_ATOMIC_HOT_WORDS; l++)
+      for (uint32_t id = 0; id <= kCount; id++) id_of[f * 32u + l][gsb_shared_atomic_exch(seed, f, l, id, 0u)] = id;
+  for (uint32_t b = 0; b < ctas; b++)
+    for (uint32_t f = 0; f < forms; f++)
+      for (uint32_t l = 0; l < GSB_SHARED_ATOMIC_HOT_WORDS; l++) {
+        std::fill(seen.begin(), seen.end(), 0);
+        const bool exch = unit == GSB_SHARED_ATOMIC_UNIT_TICKET && f > 0;
+        const uint32_t comps = exch ? (f == 1u ? 1u : f == 2u ? 2u : 4u) : 1u;
+        for (uint32_t i = 0; i < (exch ? kCount + 1u : kCount); i++) {
+          const uint32_t *e = &slots[gsb_shared_atomic_slot(b, f, l, i)];
+          uint32_t id = e[0];
+          if (exch) {  // the id whose value this is, every component of it
+            const auto it = id_of[f * 32u + l].find(e[0]);
+            id = it == id_of[f * 32u + l].end() ? GSB_SHARED_ATOMIC_NO_ID : it->second;
+            for (uint32_t c = 1; c < comps && id != GSB_SHARED_ATOMIC_NO_ID; c++)
+              if (e[c] != gsb_shared_atomic_exch(seed, f, l, id, c)) id = GSB_SHARED_ATOMIC_NO_ID;
+          }
+          if (id <= (exch ? kCount : kCount - 1u) && !seen[id]) {
+            seen[id] = 1;
+            continue;
+          }
+          bad++;
+          const uint32_t sm = b < GSB_SM_MAX ? log.cta_smid[b] : GSB_SHARED_ATOMIC_NO_SM;
+          shared_atomic_add_record(out, {sm, unit, GSB_SHARED_ATOMIC_REC_SLOT,
+                                         (uint32_t)(gsb_shared_atomic_slot(b, f, l, i) / 4u), kCount, e[0]});
+        }
+      }
+  return bad;
+}
+
+int shared_atomic_probe_locked(Device *d, const gsb_shared_atomic_cfg *cfg, gsb_shared_atomic_result *out) {
+  const uint64_t t0 = now_ns();
+  if (cfg->units & ~kSharedAtomicAllUnits) {
+    set_error("invalid shared-memory atomic unit mask 0x%x", cfg->units);
+    return out->status = GSB_ERR_INVALID_ARGUMENT;
+  }
+  out->units = cfg->units ? cfg->units : kSharedAtomicAllUnits;
+  out->sm_count = d->sm_count;
+  for (gsb_shared_atomic_run &run : out->run) run.hook_cta = GSB_SHARED_ATOMIC_NO_SM;
+  int rc = ensure_ready(d);
+  if (!rc) rc = sm_drain_kept_locked(d);
+  if (rc) return out->status = rc;
+  if (d->sm_count > GSB_SM_MAX) {
+    set_error("%s has %u SMs, more than the shared-memory atomic probe's %d", d->uuid, d->sm_count, GSB_SM_MAX);
+    return out->status = GSB_ERR_INVALID_ARGUMENT;
+  }
+  int smem = 0;
+  if ((rc = smem_optin_locked(d, &smem))) return out->status = rc;
+  out->seed = seed_or_fresh(cfg->seed, 0x53410000u, &d->shared_atomic.seed);
+  out->seed_expect = cfg->seed_expect ? cfg->seed_expect : out->seed;
+  const Device::SharedAtomicHooks hooks = take_hooks(d, &d->shared_atomic.hooks);
+  // DSMEM and REDAS: clusters of 2, then the largest of 16 and 8 that can be scheduled, as many as fit at once
+  const bool any_cluster = out->units >> GSB_SHARED_ATOMIC_UNIT_DSMEM & 1u || out->units >> GSB_SHARED_ATOMIC_UNIT_REDAS & 1u;
+  uint32_t max_clusters[2][2] = {};  // [DSMEM, REDAS][size]
+  if (any_cluster) {
+    const auto fit = [&](uint32_t u, uint32_t n) {
+      int m = 0;
+      if (gsb_shared_atomic_max_clusters(u, n, smem, &m) != cudaSuccess) {
+        cudaGetLastError();
+        m = 0;
+      }
+      return (uint32_t)std::max(0, std::min(m, (int)(GSB_SM_MAX / n)));
+    };
+    const uint32_t big = fit(GSB_SHARED_ATOMIC_UNIT_DSMEM, 16u) ? 16u : fit(GSB_SHARED_ATOMIC_UNIT_DSMEM, 8u) ? 8u : 0u;
+    out->cluster_n[0] = 2u;
+    out->cluster_n[1] = big;
+    for (uint32_t c = 0; c < 2; c++)
+      for (uint32_t k = 0; k < 2; k++)
+        max_clusters[c][k] = out->cluster_n[k] ? fit(GSB_SHARED_ATOMIC_UNIT_DSMEM + c, out->cluster_n[k]) : 0u;
+  }
+  // one transient buffer: the launch log, every local unit's expected area, DSMEM's and REDAS's areas by cluster size
+  // and rank (16 each), the TICKET and CAS slots
+  const uint32_t ctas = d->sm_count;
+  const size_t area = (size_t)GSB_SHARED_ATOMIC_AREA_WORDS * 4u;
+  constexpr uint32_t kLocal = GSB_SHARED_ATOMIC_UNIT_DSMEM;  // units 0 .. kLocal - 1 run one CTA per SM
+  const auto area_index = [&](uint32_t u, uint32_t k, uint32_t rank) {
+    return u < kLocal ? (size_t)u : kLocal + ((size_t)(u - kLocal) * 2u + k) * 16u + rank;
+  };
+  const size_t n_areas = kLocal + 2u * 2u * 16u;
+  const size_t off_expect = kSharedAtomicLogBytes, off_slots = off_expect + n_areas * area;
+  const bool any_slots = out->units >> GSB_SHARED_ATOMIC_UNIT_TICKET & 1u || out->units >> GSB_SHARED_ATOMIC_UNIT_CAS & 1u;
+  const size_t slot_words = any_slots ? (size_t)ctas * GSB_SHARED_ATOMIC_SLOT_WORDS : 0u;
+  const size_t bytes = off_slots + 4u * slot_words;
+  std::vector<uint32_t> expect(n_areas * GSB_SHARED_ATOMIC_AREA_WORDS);
+  const uint64_t t_exp = now_ns();
+  for (uint32_t u = 0; u < GSB_SHARED_ATOMIC_UNITS; u++) {
+    if (!(out->units >> u & 1u)) continue;
+    for (uint32_t k = 0; k < (u < kLocal ? 1u : 2u); k++) {
+      const uint32_t n = u < kLocal ? 1u : out->cluster_n[k];
+      for (uint32_t rank = 0; rank < n; rank++)
+        if (gsb_shared_atomic_expected(u, out->seed_expect, n, rank,
+                                       &expect[area_index(u, k, rank) * GSB_SHARED_ATOMIC_AREA_WORDS],
+                                       GSB_SHARED_ATOMIC_AREA_WORDS) != GSB_SHARED_ATOMIC_AREA_WORDS) {
+          set_error("computing the shared-memory atomic probe's expected words of unit %u on %s", u, d->uuid);
+          return out->status = GSB_ERR_INVALID_ARGUMENT;
+        }
+    }
+  }
+  out->expected_ns = now_ns() - t_exp;
+  SmBuffer buf(d, rc);
+  rc = buf.alloc("shared-memory atomic probe", bytes);
+  char *const base = static_cast<char *>(buf.p);
+  if (rc == GSB_OK) {
+    cudaError_t e = cudaMemcpyAsync(base + off_expect, expect.data(), 4u * expect.size(), cudaMemcpyHostToDevice, d->stream);
+    if (e == cudaSuccess) e = cudaStreamSynchronize(d->stream);
+    if (e != cudaSuccess) {
+      set_error("uploading the shared-memory atomic probe's expected words to %s: %s", d->uuid, cudaGetErrorString(e));
+      rc = GSB_ERR_DRIVER;
+    }
+  }
+  bool first = true;
+  std::vector<uint32_t> slots;
+  for (uint32_t u = 0; u < GSB_SHARED_ATOMIC_UNITS && rc == GSB_OK; u++) {
+    if (!(out->units >> u & 1u)) continue;
+    gsb_shared_atomic_run &run = out->run[u];
+    const bool tickets = u == GSB_SHARED_ATOMIC_UNIT_TICKET || u == GSB_SHARED_ATOMIC_UNIT_CAS;
+    const bool cluster = u >= kLocal;
+    gsb_shared_atomic_args a;
+    memset(&a, 0, sizeof a);
+    a.log = reinterpret_cast<gsb_shared_atomic_log *>(base);
+    a.slots = tickets ? reinterpret_cast<uint32_t *>(base + off_slots) : nullptr;
+    a.seed = out->seed;
+    a.smem_bytes = (uint32_t)smem;
+    // a CAS loop or a REDAS wait may run to its deadline (one per thread, one per CTA)
+    const uint64_t extra_ms =
+        u == GSB_SHARED_ATOMIC_UNIT_CAS || cluster ? GSB_SHARED_ATOMIC_CAS_WAIT_NS / 1000000u : 0u;
+    uint32_t covered[GSB_SM_MAX / 32] = {0};
+    for (uint32_t k = 0; k < (cluster ? 2u : 1u) && rc == GSB_OK; k++) {
+      const uint32_t n = cluster ? out->cluster_n[k] : 1u;
+      const uint32_t clusters = cluster ? max_clusters[u - kLocal][k] : ctas;
+      if (cluster && !clusters) {
+        if (k == 0) {  // not even clusters of 2 can be scheduled: nothing of the unit can run
+          set_error("clusters of 2 CTAs with %d bytes of shared memory each cannot be scheduled on %s", smem, d->uuid);
+          run.status = rc = GSB_ERR_UNSUPPORTED_ARCH;
+        }
+        continue;
+      }
+      a.expected = reinterpret_cast<const uint32_t *>(base + off_expect + area_index(u, k, 0) * area);
+      const uint32_t reach = std::min(clusters * n, ctas);
+      uint32_t size_covered[GSB_SM_MAX / 32] = {0}, launches = 0;
+      if (cluster) run.clusters[k] = clusters;
+      // a launch that left an SM it could reach uncovered (another context held it) is repeated
+      while (launches < GSB_SHARED_ATOMIC_MAX_LAUNCHES && popcount_bitmap(size_covered) < reach) {
+        const bool first_launch = run.launches == 0;  // test hooks: the unit's first launch only
+        a.hook_smid = first_launch && hooks.corrupt[u].armed ? hooks.corrupt[u].smid : GSB_SM_MAX;
+        a.hook_index = hooks.corrupt[u].index;
+        a.hook_xr = hooks.corrupt[u].xr;
+        a.skip_smid = first_launch && hooks.skip[u].armed ? hooks.skip[u].smid : GSB_SM_MAX;
+        run.launches++;
+        launches++;
+        if (cluster) run.cluster_launches[k]++;
+        gsb_shared_atomic_log log;
+        int lrc = sm_launch_locked(
+            d, "shared-memory atomic check",
+            [&] {
+              return cluster ? gsb_shared_atomic_cluster_launch(u, n, clusters, &a, d->stream)
+                             : gsb_shared_atomic_kernel_launch(u, ctas, &a, d->stream);
+            },
+            a.log, &log, sizeof log, extra_ms, nullptr, &run.kernel_ns);
+        if (lrc == GSB_OK && tickets) {
+          slots.resize(slot_words);
+          const cudaError_t e = cudaMemcpy(slots.data(), a.slots, 4u * slots.size(), cudaMemcpyDeviceToHost);
+          if (e != cudaSuccess) {
+            set_error("reading the shared-memory atomic probe's slots on %s: %s", d->uuid, cudaGetErrorString(e));
+            lrc = GSB_ERR_DRIVER;
+          }
+        }
+        if (lrc != GSB_OK) {
+          run.status = rc = lrc;
+          break;
+        }
+        if (log.skipped_cta) run.hook_cta = log.skipped_cta - 1u;
+        run.atomics_issued += log.issued;
+        run.timeouts += log.timeouts;
+        run.cas_max_ns = std::max<uint64_t>(run.cas_max_ns, log.cas_max_ns);
+        run.ticket_faults += log.faults;
+        // records: the kernel's (out-of-range tickets, torn pairs, wrong words), then slots
+        fold_log(log, &run, out, size_covered);
+        if (tickets) run.ticket_faults += shared_atomic_check_slots(u, out->seed_expect, ctas, slots, log, out);
+      }
+      for (int i = 0; i < GSB_SM_MAX / 32; i++) covered[i] |= size_covered[i];
+    }
+    run.sms_covered = popcount_bitmap(covered);
+    for (int i = 0; i < GSB_SM_MAX / 32; i++) out->covered[i] = first ? covered[i] : out->covered[i] & covered[i];
+    first = false;
+  }
+  out->sms_covered = popcount_bitmap(out->covered);
+  buf.release();
+  out->wall_ns = now_ns() - t0;
+  out->status = rc;
+  bool ran = false, short_cover = false;
+  for (const gsb_shared_atomic_run &run : out->run) {
+    ran = ran || run.launches != 0;
+    short_cover = short_cover || (run.launches != 0 && run.status == GSB_OK && run.sms_covered < out->sm_count);
+  }
+  count_probe(d, &d->shared_atomic.stats, *out, ran, gsb_shared_atomic_conditions(out),
+              short_cover ? &d->shared_atomic.stats.incomplete : nullptr);
+  return rc;
+}
+
 // ------------------------------------------------------------------ the periodic checks, described once
 
 template <typename Run>
@@ -3671,10 +3903,12 @@ using OrderCheck = Check<GSB_OPT_ORDER_PROBE_EVERY_CYCLES, GSB_EVENT_ORDER, &Dev
                          &gsb_order_conditions>;
 using SparseCheck = Check<GSB_OPT_SPARSE_PROBE_EVERY_CYCLES, GSB_EVENT_SPARSE, &Device::sparse, &sparse_probe_locked,
                           &gsb_sparse_conditions>;
+using SharedAtomicCheck = Check<GSB_OPT_SHARED_ATOMIC_PROBE_EVERY_CYCLES, GSB_EVENT_SHARED_ATOMIC, &Device::shared_atomic,
+                                &shared_atomic_probe_locked, &gsb_shared_atomic_conditions>;
 // in the order the prober runs them when several are due after the same cycle; G.check_every follows it
 using Checks =
     std::tuple<LinkCheck, CopyCheck, SmCheck, ClusterCheck, AtomicCheck, TensorCheck, SfuCheck, L1Check, OrderCheck,
-               SparseCheck>;
+               SparseCheck, SharedAtomicCheck>;
 static_assert(std::tuple_size<Checks>::value == std::extent<decltype(G.check_every)>::value, "one cadence per check");
 
 // f(check, its place in Checks) for every periodic check, in order
@@ -4664,6 +4898,41 @@ uint64_t tensor_word_mask(uint32_t unit) {
 }  // namespace
 
 extern "C" {
+
+int gsb_shared_atomic_probe(uint32_t idx, const gsb_shared_atomic_cfg *cfg, gsb_shared_atomic_result *out) {
+  return probe_entry(idx, cfg, out, &SharedAtomicCheck::run);
+}
+
+int gsb_shared_atomic_stats_get(uint32_t idx, gsb_shared_atomic_stats *out) {
+  return stats_entry(idx, out, [](Device *d) { return &d->shared_atomic.stats; });
+}
+
+int gsb_test_shared_atomic_corrupt(uint32_t idx, uint32_t smid, uint32_t unit, uint32_t index, uint64_t xr) {
+  std::shared_lock<std::shared_mutex> api_lk(G.api_mu);
+  if (unit >= GSB_SHARED_ATOMIC_UNITS || smid >= GSB_SM_MAX || index >= GSB_SHARED_ATOMIC_AREA_WORDS || (xr >> 32))
+    return GSB_ERR_INVALID_ARGUMENT;
+  Device *d = device_at(idx);
+  if (!d) return G.inited ? GSB_ERR_NO_DEVICE : GSB_ERR_NOT_INITIALIZED;
+  std::lock_guard<std::mutex> lk(d->smu);
+  Device::SmCorrupt &c = d->shared_atomic.hooks.corrupt[unit];
+  c.armed = true;
+  c.smid = smid;
+  c.index = index;
+  c.xr = xr;
+  return GSB_OK;
+}
+
+int gsb_test_shared_atomic_skip(uint32_t idx, uint32_t smid, uint32_t unit) {
+  std::shared_lock<std::shared_mutex> api_lk(G.api_mu);
+  if (unit >= GSB_SHARED_ATOMIC_UNITS || smid >= GSB_SM_MAX) return GSB_ERR_INVALID_ARGUMENT;
+  Device *d = device_at(idx);
+  if (!d) return G.inited ? GSB_ERR_NO_DEVICE : GSB_ERR_NOT_INITIALIZED;
+  std::lock_guard<std::mutex> lk(d->smu);
+  Device::SmCorrupt &c = d->shared_atomic.hooks.skip[unit];
+  c.armed = true;
+  c.smid = smid;
+  return GSB_OK;
+}
 
 int gsb_sparse_probe(uint32_t idx, const gsb_sparse_cfg *cfg, gsb_sparse_result *out) {
   return probe_entry(idx, cfg, out, &SparseCheck::run);

@@ -423,4 +423,50 @@ int gsb_atomic_kernel_preload(int smem_bytes);
 int gsb_atomic_values_launch(const gsb_atomic_args *a, const uint64_t *values, cudaStream_t stream);
 int gsb_atomic_values_preload(int smem_bytes);
 
+/* What one shared-memory atomic launch (shared_atomic_check_sm90a.cu, libgpushare_b200_shared_atomic.so) leaves in
+ * device memory; the host zeroes it before every launch. Its leading fields are the SM check's, so fold_log serves it. */
+struct gsb_shared_atomic_log {
+  unsigned int covered[GSB_SM_MAX / 32]; /* bit %smid: a CTA of the launch ran there */
+  unsigned int faulty[GSB_SM_MAX / 32];  /* bit %smid: a wrong word or an out-of-range ticket there */
+  unsigned long long words;              /* area words compared */
+  unsigned long long mismatch_words;
+  unsigned long long mismatch_bits;
+  unsigned int count;                    /* records claimed (may pass GSB_SHARED_ATOMIC_RECORDS) */
+  unsigned int skipped_cta;              /* blockIdx + 1 of the CTA that applied the skip hook; 0: none */
+  unsigned long long issued;             /* atomics issued (CAS: successful swaps) */
+  unsigned int timeouts;                 /* CAS loops and REDAS waits that ran out */
+  unsigned int faults;                   /* tickets returned at or past the count, torn b128 pairs */
+  unsigned int cas_max_ns;               /* the longest CAS loop */
+  unsigned int reserved0;
+  unsigned int cta_smid[GSB_SM_MAX];     /* %smid of each CTA, by blockIdx */
+  gsb_shared_atomic_record rec[GSB_SHARED_ATOMIC_RECORDS];
+};
+
+struct gsb_shared_atomic_args {
+  gsb_shared_atomic_log *log;
+  const uint32_t *expected;   /* GSB_SHARED_ATOMIC_AREA_WORDS: every CTA's area after a clean run (DSMEM, REDAS: one
+                                 area per cluster rank) */
+  uint32_t *slots;            /* TICKET, CAS: grid x GSB_SHARED_ATOMIC_SLOT_WORDS (gsb_shared_atomic_slot) */
+  unsigned long long hook_xr; /* test hook: XORed into observed word hook_index by the CTA on hook_smid */
+  uint32_t seed;              /* the starting words and the contributions */
+  uint32_t hook_smid;         /* GSB_SM_MAX: no corrupt hook */
+  uint32_t hook_index;
+  uint32_t skip_smid;         /* test hook: the CTA on this SM issues no atomic; GSB_SM_MAX: none */
+  uint32_t smem_bytes;        /* dynamic shared memory of every CTA */
+  uint32_t reserved0;
+};
+
+/* Enqueue one shared-memory atomic launch of GSB_SHARED_ATOMIC_UNIT_* `unit` with `grid` CTAs on `stream`. Returns
+ * cudaError_t as int. */
+int gsb_shared_atomic_kernel_launch(uint32_t unit, uint32_t grid, const gsb_shared_atomic_args *a, cudaStream_t stream);
+/* Enqueue one DSMEM or REDAS launch: `clusters` clusters of n CTAs on `stream`; a->expected holds the n ranks' areas.
+ * Returns cudaError_t as int. */
+int gsb_shared_atomic_cluster_launch(uint32_t unit, uint32_t n, uint32_t clusters, const gsb_shared_atomic_args *a,
+                                     cudaStream_t stream);
+/* cudaOccupancyMaxActiveClusters of `unit`'s clusters of n CTAs with `smem_bytes` each (0 when none fits). */
+int gsb_shared_atomic_max_clusters(uint32_t unit, uint32_t n, int smem_bytes, int *clusters);
+/* Load its kernels into the CURRENT context, let each take `smem_bytes` of dynamic shared memory and allow clusters of
+ * 16. */
+int gsb_shared_atomic_kernel_preload(int smem_bytes);
+
 #endif /* GSB_INTERNAL_H_ */

@@ -878,6 +878,69 @@ test_sparse_corrupt.__test__ = False
 test_sparse_operands.__test__ = False
 
 
+def shared_atomic_probe(idx: int, *, seed: int = 0, seed_expect: int = 0, units: int = 0,
+                        raise_on_error: bool = True) -> "_abi.SharedAtomicResult":
+    """Shared-memory atomic probe of device `idx`: each unit (`units`: a mask of 1 << GSB_SHARED_ATOMIC_UNIT_*, 0 =
+    all) on every SM, its area compared bit for bit with the words for `seed_expect` (0 = `seed`; `seed` 0 = fresh).
+    Mismatches and slot faults are a result, not an error; with raise_on_error=False a failed launch is too
+    (``status`` < 0)."""
+    cfg = _abi.SharedAtomicCfg(units, seed, seed_expect, 0)
+    r = _abi.SharedAtomicResult()
+    rc = lib.gsb_shared_atomic_probe(idx, C.byref(cfg), C.byref(r))
+    if raise_on_error:
+        check(rc, f"gsb_shared_atomic_probe({idx})")
+    return r
+
+
+def shared_atomic_stats(idx: int) -> "_abi.SharedAtomicStats":
+    """Shared-memory atomic probes of device `idx` since health_start: count, faults, skipped, incomplete, the last
+    result."""
+    st = _abi.SharedAtomicStats()
+    check(lib.gsb_shared_atomic_stats_get(idx, C.byref(st)), f"gsb_shared_atomic_stats_get({idx})")
+    return st
+
+
+def shared_atomic_expected(unit: int, seed: int, cluster: int = 1, rank: int = 0) -> List[int]:
+    """The 3072 4-byte words of one CTA's area after a clean run of shared-memory atomic unit `unit` under `seed`
+    (DSMEM, REDAS: of rank `rank` of a cluster of `cluster` CTAs)."""
+    n = check(int(lib.gsb_shared_atomic_expected(unit, seed, cluster, rank, None, 0)),
+              "gsb_shared_atomic_expected(size)")
+    out = (C.c_uint32 * n)()
+    check(int(lib.gsb_shared_atomic_expected(unit, seed, cluster, rank, out, n)), "gsb_shared_atomic_expected")
+    return list(out)
+
+
+def shared_atomic_conditions(r: "_abi.SharedAtomicResult") -> int:
+    """GSB_SHARED_ATOMIC_* bits a shared-memory atomic probe result raises."""
+    return lib.gsb_shared_atomic_conditions(C.byref(r))
+
+
+def shared_atomic_text(r: "_abi.SharedAtomicResult", uuid: str) -> str:
+    """The one log line both daemons print for a shared-memory atomic probe result."""
+    need = lib.gsb_shared_atomic_text(C.byref(r), uuid.encode(), None, 0)
+    check(int(need), "gsb_shared_atomic_text(size)")
+    buf = C.create_string_buffer(int(need))
+    n = lib.gsb_shared_atomic_text(C.byref(r), uuid.encode(), buf, int(need))
+    check(int(n), "gsb_shared_atomic_text")
+    return buf.raw[: int(n)].decode()
+
+
+def test_shared_atomic_corrupt(idx: int, smid: int, unit: int, index: int, xr: int) -> None:
+    """Test hook: on the next shared-memory atomic probe of `idx`, in the first launch of `unit`, the CTA on SM `smid`
+    XORs `xr` into its area word `index` just before the compare; once."""
+    check(lib.gsb_test_shared_atomic_corrupt(idx, smid, unit, index, xr), f"gsb_test_shared_atomic_corrupt({idx})")
+
+
+def test_shared_atomic_skip(idx: int, smid: int, unit: int) -> None:
+    """Test hook: on the next shared-memory atomic probe of `idx`, in the first launch of `unit`, the CTA on SM `smid`
+    issues none of the unit's atomics; once."""
+    check(lib.gsb_test_shared_atomic_skip(idx, smid, unit), f"gsb_test_shared_atomic_skip({idx})")
+
+
+test_shared_atomic_corrupt.__test__ = False
+test_shared_atomic_skip.__test__ = False
+
+
 def sfu_probe(idx: int, *, seed: int = 0, seed_expect: int = 0, units: int = 0,
               raise_on_error: bool = True) -> "_abi.SfuResult":
     """SM special-function probe of device `idx`: every instruction of each unit (`units`: a mask of

@@ -24,7 +24,8 @@ from .._abi import (COPY_CONDITION_NAMES, ECC_CONDITION_NAMES, GSB_EVENT_COPY, G
                     GSB_OPT_SFU_PROBE_EVERY_CYCLES, SfuResult, L1_CONDITION_NAMES, GSB_EVENT_L1,
                     GSB_OPT_L1_PROBE_EVERY_CYCLES, L1Result, ORDER_CONDITION_NAMES, GSB_EVENT_ORDER,
                     GSB_OPT_ORDER_PROBE_EVERY_CYCLES, OrderResult, SPARSE_CONDITION_NAMES, GSB_EVENT_SPARSE,
-                    GSB_OPT_SPARSE_PROBE_EVERY_CYCLES, SparseResult)
+                    GSB_OPT_SPARSE_PROBE_EVERY_CYCLES, SparseResult, SHARED_ATOMIC_CONDITION_NAMES,
+                    GSB_EVENT_SHARED_ATOMIC, GSB_OPT_SHARED_ATOMIC_PROBE_EVERY_CYCLES, SharedAtomicResult)
 from . import const
 
 log = logging.getLogger("gpushare.nvidia")
@@ -159,6 +160,9 @@ CHECKS = (
           ORDER_CONDITION_NAMES, "memory-ordering health", "memory-ordering"),
     Check(GSB_OPT_SPARSE_PROBE_EVERY_CYCLES, GSB_EVENT_SPARSE, device.sparse_stats, device.sparse_text, SparseResult,
           SPARSE_CONDITION_NAMES, "sparse tensor-core health", "sparse"),
+    Check(GSB_OPT_SHARED_ATOMIC_PROBE_EVERY_CYCLES, GSB_EVENT_SHARED_ATOMIC, device.shared_atomic_stats,
+          device.shared_atomic_text, SharedAtomicResult, SHARED_ATOMIC_CONDITION_NAMES, "shared-memory atomic health",
+          "shared-atomic"),
 )
 
 
@@ -180,7 +184,7 @@ def watchXIDs(stop: threading.Event, devs: List[Device], xids: Callable[[List[De
               recovered: Optional[Callable[[Device], None]] = None, recovery_cycles: int = 0,
               ecc: bool = False, link_every: int = 0, copy_every: int = 0, sm_every: int = 0,
               cluster_every: int = 0, atomic_every: int = 0, tensor_every: int = 0, sfu_every: int = 0,
-              l1_every: int = 0, order_every: int = 0, sparse_every: int = 0) -> None:
+              l1_every: int = 0, order_every: int = 0, sparse_every: int = 0, shared_atomic_every: int = 0) -> None:
     """nvidia.go:100-152 with the event source replaced: gsb_health_wait delivers both XID critical
     errors (same NVML event type, registered once per GPU) and verdicts of the active HBM probe.
     The loop shape, the 5 s wait, the XID 31/43/45 filter, "empty UUID = every device" and "every
@@ -193,12 +197,13 @@ def watchXIDs(stop: threading.Event, devs: List[Device], xids: Callable[[List[De
     L2 atomic probe `atomic_every` (not in the reference) > 0 runs, of the tensor-core format probe `tensor_every`
     (not in the reference) > 0 runs, of the SM special-function probe `sfu_every` (not in the reference) > 0 runs,
     of the L1 and constant-cache probe `l1_every` (not in the reference) > 0 runs, of the memory-ordering probe
-    `order_every` (not in the reference) > 0 runs and of the sparse tensor-core probe `sparse_every` (not in the
-    reference) > 0 runs."""
+    `order_every` (not in the reference) > 0 runs, of the sparse tensor-core probe `sparse_every` (not in the
+    reference) > 0 runs and of the shared-memory atomic probe `shared_atomic_every` (not in the reference) > 0
+    runs."""
     lib.gsb_health_set_recovery(recovery_cycles if recovered is not None else 0)
     device.set_option(GSB_OPT_ECC_HEALTH, 1 if ecc else 0)
     every = dict(zip(CHECKS, (link_every, copy_every, sm_every, cluster_every, atomic_every, tensor_every, sfu_every,
-                              l1_every, order_every, sparse_every)))
+                              l1_every, order_every, sparse_every, shared_atomic_every)))
     for check, n in every.items():
         device.set_option(check.option, max(0, n))
     device.health_start(probe_period_ms, window_bytes)

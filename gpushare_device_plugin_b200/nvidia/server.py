@@ -41,7 +41,7 @@ class NvidiaDevicePlugin:
                  probe_copy_every: int = 0, probe_sm_every: int = 0, startup_stress_ms: int = 0,
                  probe_cluster_every: int = 0, probe_atomic_every: int = 0, probe_tensor_every: int = 0,
                  probe_sfu_every: int = 0, probe_l1_every: int = 0, probe_order_every: int = 0,
-                 probe_sparse_every: int = 0):
+                 probe_sparse_every: int = 0, probe_shared_atomic_every: int = 0):
         # `inventory` = (devs, devNameMap) injects a synthetic node (tests, Allocate benchmark)
         self.devs, self.devNameMap = inventory if inventory is not None else nvidia.getDevices()  # server.go:39
         devList = list(self.devNameMap)
@@ -71,6 +71,7 @@ class NvidiaDevicePlugin:
         self.probe_l1_every = probe_l1_every
         self.probe_order_every = probe_order_every
         self.probe_sparse_every = probe_sparse_every
+        self.probe_shared_atomic_every = probe_shared_atomic_every
         self.startup_stress_ms = startup_stress_ms
         self.max_workers = max_workers
         self.stop = threading.Event()
@@ -284,7 +285,8 @@ class NvidiaDevicePlugin:
                              self.recovered, self.health_recovery_cycles, self.health_ecc, self.probe_link_every,
                              self.probe_copy_every, self.probe_sm_every, self.probe_cluster_every,
                              self.probe_atomic_every, self.probe_tensor_every, self.probe_sfu_every,
-                             self.probe_l1_every, self.probe_order_every, self.probe_sparse_every)
+                             self.probe_l1_every, self.probe_order_every, self.probe_sparse_every,
+                             self.probe_shared_atomic_every)
         else:
             self.stop.wait()
 

@@ -49,7 +49,8 @@ extern "C" {
                               (gsb_l1_*, GSB_EVENT_L1) likewise, found by gsb_l1_probe; memory-ordering health
                               (gsb_order_*, GSB_EVENT_ORDER) likewise, found by gsb_order_probe; sparse
                               tensor-core health (gsb_sparse_*, GSB_EVENT_SPARSE) likewise, found by
-                              gsb_sparse_probe */
+                              gsb_sparse_probe; shared-memory atomic health (gsb_shared_atomic_*,
+                              GSB_EVENT_SHARED_ATOMIC) likewise, found by gsb_shared_atomic_probe */
 
 /* = NVML_DEVICE_UUID_BUFFER_SIZE (vendor/.../nvml/nvml.h:1567), used by bindings.go:20 szUUID */
 #define GSB_UUID_BUFFER_SIZE 80
@@ -178,10 +179,14 @@ enum {
                                             a health session and after every Nth cycle, outside gsb_cycle (after the
                                             link to L1 probes when they are due), and raises GSB_EVENT_ORDER; 0 = off
                                             (default): no buffer, no launch */
-  GSB_OPT_SPARSE_PROBE_EVERY_CYCLES = 17  /* N > 0: each prober thread runs gsb_sparse_probe after its first cycle of
-                                            a health session and after every Nth cycle, outside gsb_cycle (after every
-                                            other periodic probe that is due), and raises GSB_EVENT_SPARSE; 0 = off
-                                            (default): no buffer, no launch */
+  GSB_OPT_SPARSE_PROBE_EVERY_CYCLES = 17, /* N > 0: each prober thread runs gsb_sparse_probe after its first cycle of
+                                            a health session and after every Nth cycle, outside gsb_cycle (after the
+                                            link to memory-ordering probes when they are due), and raises
+                                            GSB_EVENT_SPARSE; 0 = off (default): no buffer, no launch */
+  GSB_OPT_SHARED_ATOMIC_PROBE_EVERY_CYCLES = 18 /* N > 0: each prober thread runs gsb_shared_atomic_probe after its
+                                            first cycle of a health session and after every Nth cycle, outside
+                                            gsb_cycle (after every other periodic probe that is due), and raises
+                                            GSB_EVENT_SHARED_ATOMIC; 0 = off (default): no buffer, no launch */
 };
 enum {
   GSB_INVENTORY_SNAPSHOT = 0, /* cycle: NVML's (re)start-time answer + per-cycle CUDA-side identity check */
@@ -350,8 +355,10 @@ enum {
                                   GSB_L1_* bit */
   GSB_EVENT_ORDER = 0x80000,   /* GSB_OPT_ORDER_PROBE_EVERY_CYCLES: a memory-ordering condition; edata = one
                                   GSB_ORDER_* bit */
-  GSB_EVENT_SPARSE = 0x100000  /* GSB_OPT_SPARSE_PROBE_EVERY_CYCLES: a sparse tensor-core condition; edata = one
+  GSB_EVENT_SPARSE = 0x100000, /* GSB_OPT_SPARSE_PROBE_EVERY_CYCLES: a sparse tensor-core condition; edata = one
                                   GSB_SPARSE_* bit */
+  GSB_EVENT_SHARED_ATOMIC = 0x200000 /* GSB_OPT_SHARED_ATOMIC_PROBE_EVERY_CYCLES: a shared-memory atomic condition;
+                                        edata = one GSB_SHARED_ATOMIC_* bit */
 };
 enum { GSB_PROBE_FAULT_MISMATCH = 1, GSB_PROBE_FAULT_LAUNCH = 2, GSB_PROBE_RECOVERED = 3,
        GSB_PROBE_FAULT_WEDGED = 4 /* the launch outlived the completion watchdog */ };
@@ -2074,6 +2081,169 @@ int gsb_test_sparse_corrupt(uint32_t idx, uint32_t smid, uint32_t unit, uint32_t
  * scale outside its range, a pattern outside the unit's set, or an expected word wider than 32 bits. */
 int gsb_test_sparse_operands(uint32_t idx, uint32_t unit, const int32_t *a, const uint8_t *pattern, const int32_t *b,
                              const int32_t *sa, const int32_t *sb, const uint64_t *expected);
+
+/* ---- Shared-memory atomic health (not in the reference; opt-in: GSB_OPT_SHARED_ATOMIC_PROBE_EVERY_CYCLES) ------- */
+
+/*
+ * Bit-exact checks of the atomic unit of every SM's shared memory (ATOMS), which histograms, radix sorts, block
+ * reductions and work queues run on. Each unit is one launch of one CTA per SM (GSB_SHARED_ATOMIC_THREADS threads, the
+ * opt-in maximum of dynamic shared memory, so no two CTAs share an SM; thread 0 records %smid); a launch that left an
+ * SM uncovered is repeated up to GSB_SHARED_ATOMIC_MAX_LAUNCHES times. Each CTA writes the unit's starting words into
+ * an area of its own shared memory (GSB_SHARED_ATOMIC_AREA_BYTES: a spread region of GSB_SHARED_ATOMIC_SPREAD_BYTES,
+ * then GSB_SHARED_ATOMIC_HOT_WORDS hot slots GSB_SHARED_ATOMIC_HOT_STRIDE bytes apart), issues the unit's atomics, and
+ * after a barrier compares every word of the area bit for bit, on the SM, with words computed on the host
+ * (gsb_shared_atomic_expected) and uploaded into a transient buffer. Two phases:
+ *
+ *   spread  every thread issues one atomic in each of 2 x E rounds (E = spread bytes / 256 / unit bytes). Even rounds
+ *           reach every word once, conflict-free, each lane's bank rotating by round and warp; in odd rounds the 32
+ *           lanes of a warp hit 32 words of one bank at different addresses. Not for TICKET and CAS.
+ *   hot     lane l of every warp hits hot slot l GSB_SHARED_ATOMIC_HOT_REPS times; the 32 slots lie in one bank, so the
+ *           lanes of a warp never share an address and all warps contend on the same word.
+ *
+ * Every operand is a function of (unit, seed, thread, round or repetition), never of %smid or blockIdx, so every CTA's
+ * area ends the same. Integer add, and/or/xor and min/max commute; inc and dec take one bound per word, so every order
+ * gives the same word; float contributions are integers whose sum of magnitudes stays under the type's exact bound.
+ * TICKET and CAS write their tickets, exchanged values and final exchange words to per-CTA slots of the buffer
+ * (gsb_shared_atomic_slot in csrc/gsb_shared_atomic.h), checked on the host as permutations. Every CAS loop ends at a
+ * GSB_SHARED_ATOMIC_CAS_WAIT_NS %globaltimer deadline. The log goes to the result only, never to the HBM fault log or
+ * reports.
+ *
+ * DSMEM and REDAS run in thread-block clusters, first of 2 CTAs and then of the largest size the SM-to-SM check uses (16,
+ * or 8 where 16 cannot be scheduled), as many clusters as fit at once. Every CTA writes its area's starting words; a
+ * cluster barrier; then every thread sends its atomics to every OTHER rank's area (an address in the CTA's own rank would
+ * take the local ATOMS path), each operand a function of (unit, seed, sender rank, thread, op). REDAS's receiver arms its
+ * mbarrier with exactly the bytes its peers send before that barrier and waits for them with a
+ * GSB_SHARED_ATOMIC_CAS_WAIT_NS %globaltimer deadline; a wait that runs out is counted as a timeout and the area is
+ * checked anyway. DSMEM ends its sends with a cluster barrier. Each rank then compares its area with the words for its
+ * rank and cluster size, and a last cluster barrier keeps every CTA alive until all of its cluster have compared, so no
+ * peer can reach the shared memory of a CTA that has exited.
+ */
+enum {
+  GSB_SHARED_ATOMIC_UNIT_INT32 = 0,  /* red.shared add.u32, and/or/xor.b32, min/max .s32 and .u32, inc/dec.u32, by word */
+  GSB_SHARED_ATOMIC_UNIT_WIDE = 1,   /* red.shared add.u64, and/or/xor.b64, min.s64, max.u64, by word (8-byte words) */
+  GSB_SHARED_ATOMIC_UNIT_FLOAT = 2,  /* red.shared add.f32, add.f64, add.noftz.f16x2, add.noftz.bf16x2, by word (8-byte
+                                        words; the 32-bit forms on the low half) */
+  GSB_SHARED_ATOMIC_UNIT_TICKET = 3, /* atom.shared add.u32 of 1, exch.b32, exch.b64, exch.b128 on the hot slots */
+  GSB_SHARED_ATOMIC_UNIT_CAS = 4,    /* atom.shared cas.b32, cas.b64, cas.b128 increment loops on the hot slots */
+  GSB_SHARED_ATOMIC_UNIT_DSMEM = 5,  /* red.shared::cluster add.u32, add.u64, add.f32 and an atom.shared::cluster
+                                        cas.b32 increment loop into every other rank's area */
+  GSB_SHARED_ATOMIC_UNIT_REDAS = 6   /* red.async ... mbarrier::complete_tx::bytes add.u32, add.u64, xor.b32, max.s32,
+                                        inc.u32 into every other rank's area, completing on the receiver's mbarrier */
+};
+#define GSB_SHARED_ATOMIC_UNITS 7
+#define GSB_SHARED_ATOMIC_RECORDS 64
+#define GSB_SHARED_ATOMIC_MAX_LAUNCHES 3
+#define GSB_SHARED_ATOMIC_THREADS 256
+#define GSB_SHARED_ATOMIC_SPREAD_BYTES 8192u
+#define GSB_SHARED_ATOMIC_HOT_WORDS 32u
+#define GSB_SHARED_ATOMIC_HOT_STRIDE 128u
+#define GSB_SHARED_ATOMIC_HOT_REPS 4u
+#define GSB_SHARED_ATOMIC_AREA_BYTES (GSB_SHARED_ATOMIC_SPREAD_BYTES + GSB_SHARED_ATOMIC_HOT_WORDS * GSB_SHARED_ATOMIC_HOT_STRIDE)
+#define GSB_SHARED_ATOMIC_AREA_WORDS (GSB_SHARED_ATOMIC_AREA_BYTES / 4u) /* the 4-byte words compared and recorded */
+#define GSB_SHARED_ATOMIC_CAS_WAIT_NS 100000000u /* bound of every CAS loop: 100 ms */
+#define GSB_SHARED_ATOMIC_NO_ID 0xFFFFFFFFu      /* what a slot starts as */
+#define GSB_SHARED_ATOMIC_NO_SM 0xFFFFFFFFu
+enum {
+  GSB_SHARED_ATOMIC_REC_WORD = 0,   /* index: 4-byte word of the area (DSMEM, REDAS: rank x GSB_SHARED_ATOMIC_AREA_WORDS +
+                                       word); expected and observed: that word */
+  GSB_SHARED_ATOMIC_REC_SLOT = 1,   /* index: slot entry (gsb_shared_atomic_slot / 4); expected: the contributor count;
+                                       observed: its first word, not a distinct valid id or exchanged value */
+  GSB_SHARED_ATOMIC_REC_TICKET = 2, /* index: hot slot; expected: the count; observed: a ticket at or past it */
+  GSB_SHARED_ATOMIC_REC_TORN = 3    /* index: hot slot; a CAS.b128 returned a pair whose halves do not belong together:
+                                       expected the hash of observed's count, observed the returned upper half */
+};
+
+typedef struct gsb_shared_atomic_cfg {
+  uint32_t units;       /* mask of 1 << GSB_SHARED_ATOMIC_UNIT_*; 0 = all */
+  uint32_t seed;        /* 0 = fresh per probe */
+  uint32_t seed_expect; /* seed the expected words are computed from; 0 = seed */
+  uint32_t reserved0;
+} gsb_shared_atomic_cfg;
+
+/* One wrong word, slot, ticket or pair; smid is the SM that owns the area or slots (GSB_SHARED_ATOMIC_NO_SM: none). */
+typedef struct gsb_shared_atomic_record {
+  uint32_t smid;
+  uint32_t unit;     /* GSB_SHARED_ATOMIC_UNIT_* */
+  uint32_t kind;     /* GSB_SHARED_ATOMIC_REC_* */
+  uint32_t index;
+  uint64_t expected, observed;
+} gsb_shared_atomic_record;
+
+typedef struct gsb_shared_atomic_run {
+  int32_t status;          /* GSB_OK, or the first failed launch's gsb_status (GSB_ERR_TIMEOUT: outlived the watchdog) */
+  uint32_t launches;       /* 0 = the unit did not run */
+  uint32_t sms_covered;    /* distinct %smid over its launches */
+  uint32_t hook_cta;       /* the blockIdx that applied gsb_test_shared_atomic_skip; GSB_SHARED_ATOMIC_NO_SM: none */
+  uint32_t cluster_launches[2]; /* DSMEM, REDAS: launches of each cluster size (gsb_shared_atomic_result.cluster_n) */
+  uint32_t clusters[2];         /* and the clusters of each of those launches; 0 for the other units */
+  uint64_t atomics_issued; /* atomic instructions issued (CAS: successful swaps) */
+  uint64_t words_checked;  /* area words compared, over every CTA of every launch */
+  uint64_t mismatch_words, mismatch_bits;
+  uint64_t ticket_faults;  /* TICKET, CAS: slots without a distinct valid id or value, tickets out of range, torn pairs */
+  uint64_t timeouts;       /* CAS loops and REDAS mbarrier waits that ran out of GSB_SHARED_ATOMIC_CAS_WAIT_NS */
+  uint64_t cas_max_ns;     /* CAS: the longest loop of any thread, by %globaltimer */
+  uint64_t kernel_ns;      /* CUDA-event time of its launches */
+} gsb_shared_atomic_run;
+
+typedef struct gsb_shared_atomic_result {
+  int32_t status;          /* GSB_OK iff every unit asked for ran every launch (mismatches and faults are a result) */
+  uint32_t sm_count;       /* the device's multiProcessorCount = the grid of every launch */
+  uint32_t seed, seed_expect, units;
+  uint32_t sms_covered;    /* SMs covered by every unit that ran */
+  uint32_t covered[GSB_SM_MAX / 32];  /* their bitmap, bit smid */
+  uint32_t faulty[GSB_SM_MAX / 32];   /* SMs a record names */
+  uint32_t cluster_n[2];   /* DSMEM, REDAS: the cluster sizes run (2, then 16 or 8); 0 when no cluster unit ran */
+  gsb_shared_atomic_run run[GSB_SHARED_ATOMIC_UNITS];
+  uint32_t n_records;      /* records filled (the first GSB_SHARED_ATOMIC_RECORDS) */
+  uint32_t reserved0;
+  gsb_shared_atomic_record records[GSB_SHARED_ATOMIC_RECORDS];
+  uint64_t expected_ns;    /* host time spent on the expected words */
+  uint64_t wall_ns;        /* host time of the whole call */
+} gsb_shared_atomic_result;
+
+/* Conditions (gsb_shared_atomic_conditions), from the units that ran only. Coverage short of sm_count after the
+ * relaunches is counted (gsb_shared_atomic_stats.incomplete) and logged, never a condition. */
+enum {
+  GSB_SHARED_ATOMIC_CORRUPT = 1u, /* a final word, a slot, a ticket or a CAS pair is wrong on some SM */
+  GSB_SHARED_ATOMIC_FAILED = 2u   /* a launch failed or outlived the watchdog, or a CAS loop or REDAS wait ran out of
+                                     its deadline */
+};
+
+/* Shared-memory atomic probes of one device since gsb_health_start (counters restart with it; gsb_shared_atomic_probe
+ * calls count too). */
+typedef struct gsb_shared_atomic_stats {
+  uint64_t probes;
+  uint64_t faults;     /* probes that raised at least one GSB_SHARED_ATOMIC_* condition */
+  uint64_t skipped;    /* probes that ran no launch (the buffer was not allocatable): no condition, no event */
+  uint64_t incomplete; /* probes in which some unit covered fewer than sm_count SMs */
+  gsb_shared_atomic_result last;
+} gsb_shared_atomic_stats;
+
+/* Holds the device while it runs; each launch under the completion watchdog. A probe that cannot take its buffer
+ * returns GSB_ERR_OUT_OF_MEMORY and counts as skipped. */
+int gsb_shared_atomic_probe(uint32_t idx, const gsb_shared_atomic_cfg *cfg, gsb_shared_atomic_result *out);
+int gsb_shared_atomic_stats_get(uint32_t idx, gsb_shared_atomic_stats *out);
+/* Pure: the GSB_SHARED_ATOMIC_AREA_WORDS 4-byte words of one CTA's area after a clean run of `unit` under `seed`
+ * (little-endian, as shared memory holds them; TICKET's exchange words, which the kernel does not compare, hold their
+ * starting value): for DSMEM and REDAS the area of rank `rank` of a cluster of `cluster` CTAs (2, 4, 8 or 16), for the
+ * other units cluster 1 and rank 0. The words do not depend on the SM count. Returns the count (with out == NULL too),
+ * GSB_ERR_BUFFER_TOO_SMALL when cap is short, or GSB_ERR_INVALID_ARGUMENT for an unknown unit, a cluster size or rank
+ * the unit does not take, or a float word whose sum of magnitudes would reach its exact bound. */
+int64_t gsb_shared_atomic_expected(uint32_t unit, uint32_t seed, uint32_t cluster, uint32_t rank, uint32_t *out,
+                                   size_t cap);
+/* Pure: GSB_SHARED_ATOMIC_* bits that hold for a result (see above). */
+uint32_t gsb_shared_atomic_conditions(const gsb_shared_atomic_result *r);
+/* Pure: the one-line text both daemons log for a result. uuid may be NULL. Returns like gsb_sm_text. */
+int64_t gsb_shared_atomic_text(const gsb_shared_atomic_result *r, const char *uuid, char *buf, size_t cap);
+/* test hook: on the next gsb_shared_atomic_probe of device idx, in the first launch of `unit`, the CTA on SM `smid`
+ * XORs xr into its observed area word `index` (4-byte words) just before the compare; once. Refused before any device
+ * is touched: unit, smid or index out of range, or xr wider than 32 bits. */
+int gsb_test_shared_atomic_corrupt(uint32_t idx, uint32_t smid, uint32_t unit, uint32_t index, uint64_t xr);
+/* test hook: on the next gsb_shared_atomic_probe of device idx, in the first launch of `unit` (DSMEM, REDAS: of clusters
+ * of 2), the CTA on SM `smid` issues none of the unit's atomics (it still writes its starting words, takes part in every
+ * cluster barrier and compares its area); once. Refused before any
+ * device is touched: unit or smid out of range. */
+int gsb_test_shared_atomic_skip(uint32_t idx, uint32_t smid, uint32_t unit);
 
 /* ---- Allocate (a12, a13): wire bytes in, wire bytes out ---------------------------------- */
 

@@ -101,6 +101,7 @@ const (
 	gsbEventL1        = uint64(C.GSB_EVENT_L1)        // opt-in L1 and constant-cache health: Edata = one of the gsbL1* conditions below
 	gsbEventOrder     = uint64(C.GSB_EVENT_ORDER)     // opt-in memory-ordering health: Edata = one of the gsbOrder* conditions below
 	gsbEventSparse    = uint64(C.GSB_EVENT_SPARSE)    // opt-in sparse tensor-core health: Edata = one of the gsbSparse* conditions below
+	gsbEventSharedAtomic = uint64(C.GSB_EVENT_SHARED_ATOMIC) // opt-in shared-memory atomic health: Edata = one of the gsbSharedAtomic* conditions below
 )
 
 const (
@@ -154,6 +155,8 @@ const (
 	gsbOrderFailed    = uint64(C.GSB_ORDER_FAILED)    // a memory-ordering launch failed or outlived the watchdog
 	gsbSparseCorrupt  = uint64(C.GSB_SPARSE_CORRUPT)  // a sparse tensor-core D word differs from its exact answer on some SM
 	gsbSparseFailed   = uint64(C.GSB_SPARSE_FAILED)   // a sparse tensor-core launch failed or outlived the watchdog
+	gsbSharedAtomicCorrupt = uint64(C.GSB_SHARED_ATOMIC_CORRUPT) // a shared-memory atomic left a wrong word, slot, ticket or pair on some SM
+	gsbSharedAtomicFailed  = uint64(C.GSB_SHARED_ATOMIC_FAILED)  // a shared-memory atomic launch failed, or a CAS loop or red.async wait ran out
 )
 
 const (
@@ -677,6 +680,34 @@ func gsbSparseLine(idx uint, uuid string) string {
 	}
 	buf := make([]byte, int(need))
 	n := C.gsb_sparse_text(&st.last, cu, (*C.char)(unsafe.Pointer(&buf[0])), C.size_t(len(buf)))
+	if n < 0 {
+		return ""
+	}
+	return string(buf[:int(n)])
+}
+
+// gsbEnableSharedAtomicHealth turns on shared-memory atomic health: each prober runs gsb_shared_atomic_probe after its
+// first cycle of a session and after every `every`-th cycle. Call it before gsbHealthStart.
+func gsbEnableSharedAtomicHealth(every uint64) error {
+	return gsbErr(C.gsb_set_option(C.GSB_OPT_SHARED_ATOMIC_PROBE_EVERY_CYCLES, C.uint64_t(every)))
+}
+
+// gsbSharedAtomicLine is the one log line of GPU idx's most recent shared-memory atomic probe ("not run" when there is
+// none): what a plugin logs before marking a GPU unhealthy on a GSB_EVENT_SHARED_ATOMIC event.
+func gsbSharedAtomicLine(idx uint, uuid string) string {
+	st := (*C.gsb_shared_atomic_stats)(C.calloc(1, C.size_t(unsafe.Sizeof(C.gsb_shared_atomic_stats{}))))
+	defer C.free(unsafe.Pointer(st))
+	if C.gsb_shared_atomic_stats_get(C.uint32_t(idx), st) != C.GSB_OK {
+		*st = C.gsb_shared_atomic_stats{}
+	}
+	cu := C.CString(uuid)
+	defer C.free(unsafe.Pointer(cu))
+	need := C.gsb_shared_atomic_text(&st.last, cu, nil, 0)
+	if need <= 0 {
+		return ""
+	}
+	buf := make([]byte, int(need))
+	n := C.gsb_shared_atomic_text(&st.last, cu, (*C.char)(unsafe.Pointer(&buf[0])), C.size_t(len(buf)))
 	if n < 0 {
 		return ""
 	}
